@@ -12,7 +12,13 @@
 //   W     = weights repacked once to [tap][Cout][Cin] fp16 (K-major rows of 128 bytes).
 // Both operands land in shared memory in the canonical K-major SWIZZLE_128B layout.  A CTA is one
 // TMA producer warp and two consumer warpgroups; each consumer warpgroup owns 64 rows of the tile
-// and issues, per K = 64 stage, 4 x wgmma (M64 x N_TILE x K16) into register accumulators.
+// and issues, per tap and K = 64 chunk, 4 x wgmma (M64 x N_TILE x K16) into register accumulators.
+//
+// Y-halo tap groups: one image row of the tile (8 px x 128 B) is exactly one 1024-byte swizzle atom, so
+// taps that read the same input view at the same dx with consecutive dy share ONE activation box of
+// TILE_H + cnt - 1 rows; tap i of the group starts its A descriptor i x 1024 B further in (the swizzle
+// phase lives in address bits 7-9 and does not change).  The K loop runs (group, chunk, tap in group):
+// one A fetch per (group, chunk) into the A ring, one weight fetch per tap into the B ring.
 //
 // Precision: x ~= x_hi + x_lo, w ~= w_hi + w_lo in fp16; with SPLIT the accumulator receives
 // x_hi*w_hi + x_hi*w_lo + x_lo*w_hi (fp32 accumulate), which reproduces the fp32 reference
@@ -36,6 +42,7 @@
 
 #include <stdlib.h>
 
+#include <algorithm>
 #include <new>
 
 #include <cuda_fp8.h>
@@ -47,11 +54,16 @@ namespace {
 
 constexpr int TILE_H = 16, TILE_W = 8;          // output pixels per tile (M = 128)
 constexpr int KCHUNK = 64;                       // fp16 elements per K stage (128 B swizzle span)
-constexpr int A_BYTES = 128 * 128;
+constexpr int ROW_BYTES = TILE_W * 128;          // one image row of an A box = one SWIZZLE_128B atom
 constexpr int MAX_TAPS = 49;
+constexpr int MAX_GROUP = 8;                     // taps per y-halo group: A boxes of at most TILE_H + 7 rows
+constexpr int RING_BYTES = 200 * 1024;           // A ring + B ring
+constexpr int MAX_STAGES = 8;                    // entries per ring
 constexpr int NUM_CONSUMERS = 256;               // warps 0..7: two consumer warpgroups
 constexpr int NUM_THREADS = NUM_CONSUMERS + 32;  // warp 8: TMA producer
 constexpr int MAX_N_TILE = 128;                  // 64 fp32 accumulator registers per consumer thread
+static_assert(2 * 2 * (TILE_H + MAX_GROUP - 1) * ROW_BYTES + 2 * 2 * MAX_N_TILE * 128 <= RING_BYTES,
+              "every plan needs two A and two B entries in the ring");
 
 // InstanceNorm (+ReLU, +residual, +LWB warp-add) fused into the conv epilogue (k_conv_wg<.., FUSED = true>): the operands
 // of the NEXT layer leave the kernel directly, no fp32 raw tensor and no second pass over HBM.  See epilogue_fused.
@@ -77,6 +89,10 @@ struct ConvParams {
     int ntaps, chunks0, chunks1;
     signed char dy[MAX_TAPS], dx[MAX_TAPS], tmap[MAX_TAPS];
     short wtap[MAX_TAPS];
+    int ngroups;                      // y-halo groups: taps g_first .. g_first + g_cnt - 1, dy consecutive (group_taps)
+    signed char g_first[MAX_TAPS], g_cnt[MAX_TAPS];
+    int a_rows;                       // A box height: TILE_H + longest group - 1
+    int a_stages, b_stages;           // ring depths inside RING_BYTES (pick_rings)
     float* out; int out_h, out_w, cout;
     int oy_mul, oy_add, ox_mul, ox_add;
     double* stats;
@@ -85,17 +101,17 @@ struct ConvParams {
                                       // (ph >> 1, ph & 1) of output pixel (2y + a, 2x + b), channel = col % phase_cols
 };
 
+// Shared memory: [A ring: a_stages x (hi | lo) boxes of a_rows rows][B ring: b_stages x (hi | lo) weight tiles] inside
+// RING_BYTES, then the barriers, the statistics partials and (fused mode) the per-channel scale / shift.
 template <int N_TILE, bool SPLIT>
 struct Cfg {
     static constexpr int B_BYTES = N_TILE * 128;
-    static constexpr int STAGE_BYTES = (A_BYTES + B_BYTES) * (SPLIT ? 2 : 1);
-    static constexpr int STAGES_RAW = (200 * 1024) / STAGE_BYTES;
-    static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-    static constexpr int BAR_BYTES = 256;
+    static constexpr int B_STAGE_BYTES = B_BYTES * (SPLIT ? 2 : 1);
+    static constexpr int BAR_BYTES = 4 * MAX_STAGES * 8;         // A full / empty, B full / empty
     static constexpr int STATS_BYTES = 8 * N_TILE * 8;           // [8 consumer warps][N_TILE] float2
     static constexpr int SS_BYTES = N_TILE * 8;                  // [N_TILE] (scale, shift), fused mode
-    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + BAR_BYTES + STATS_BYTES + SS_BYTES;
-    static_assert(STAGES >= 2, "need at least two pipeline stages");
+    static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + STATS_BYTES + SS_BYTES;
+    static_assert(B_STAGE_BYTES % 1024 == 0, "B entries must keep the 1024-byte swizzle alignment");
     static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the shared memory of a block");
 };
 
@@ -427,7 +443,7 @@ __device__ __forceinline__ void epilogue_fused(const ConvParams& P, float* acc, 
 
 // ----------------------------------------------------------------------------------- kernel
 // Operand modes (lwb_conv_desc.split): one fp16 product, the three fp16 products of the hi/lo split, or the fp16 hi
-// product + one e4m3 wgmma on the lo pair blocks (stages then hold [A_hi | A_lo8 | B_hi | B_lo8]).
+// product + one e4m3 wgmma on the lo pair blocks (A entries then hold [A_hi | A_lo8], B entries [B_hi | B_lo8]).
 enum { MODE_FP16 = 0, MODE_FP16X3 = 1, MODE_F8 = 2 };
 
 template <int N_TILE, int MODE, bool FUSED>
@@ -437,17 +453,23 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
     using C = Cfg<N_TILE, SPLIT>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-    uint64_t* bar_empty = bar_full + C::STAGES;
-    float2* s_stats = reinterpret_cast<float2*>(smem + C::STAGES * C::STAGE_BYTES + C::BAR_BYTES);   // [8][N_TILE]
-    float2* s_ss = s_stats + 8 * N_TILE;                                                             // [N_TILE]
+    const int a_op_bytes = P.a_rows * ROW_BYTES;                     // one operand (hi or lo) of an A entry
+    const int a_stage_bytes = a_op_bytes * (SPLIT ? 2 : 1);
+    uint8_t* b_ring = smem + P.a_stages * a_stage_bytes;
+    uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + RING_BYTES);
+    uint64_t* a_empty = a_full + MAX_STAGES;
+    uint64_t* b_full = a_empty + MAX_STAGES;
+    uint64_t* b_empty = b_full + MAX_STAGES;
+    float2* s_stats = reinterpret_cast<float2*>(smem + RING_BYTES + C::BAR_BYTES);   // [8][N_TILE]
+    float2* s_ss = s_stats + 8 * N_TILE;                                             // [N_TILE]
 
     const int warp = threadIdx.x >> 5;
     const unsigned lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        // empty[s] collects one arrival per consumer warp once its wgmma reads of the stage have retired
-        for (int s = 0; s < C::STAGES; s++) { mbar_init(bar_full + s, 1); mbar_init(bar_empty + s, NUM_CONSUMERS / 32); }
+        // empty[s] collects one arrival per consumer warp once its wgmma reads of the entry have retired
+        for (int s = 0; s < P.a_stages; s++) { mbar_init(a_full + s, 1); mbar_init(a_empty + s, NUM_CONSUMERS / 32); }
+        for (int s = 0; s < P.b_stages; s++) { mbar_init(b_full + s, 1); mbar_init(b_empty + s, NUM_CONSUMERS / 32); }
         fence_barrier_init();
         fence_proxy_async();
     }
@@ -458,7 +480,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
     lwb::pdl_trigger();
 
     const int nchunks = P.chunks0 + P.chunks1;
-    const int ksteps = P.ntaps * nchunks;
     const int m_tiles = P.n_img * P.tiles_y * P.tiles_x;
     const int total = m_tiles * P.n_tiles_n;
 
@@ -472,72 +493,97 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
                 asm volatile("prefetch.tensormap [%0];" :: "l"(&P.w_lo) : "memory");
             }
         }
-        int stage = 0; uint32_t phase = 0;
+        int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
         for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
             const TileCoord t = decode_tile(P, tile, m_tiles);
-            for (int s = 0; s < ksteps; s++) {
-                mbar_wait(bar_empty + stage, phase ^ 1);
-                uint8_t* st = smem + stage * C::STAGE_BYTES;
-                const int tap = s / nchunks, chunk = s % nchunks;
-                const bool second = chunk >= P.chunks0;
-                const int mi = second ? 1 : P.tmap[tap];
-                const int c0 = (second ? chunk - P.chunks0 : chunk) * KCHUNK;
-                const int xx = t.x0 + P.dx[tap], yy = t.y0 + P.dy[tap];
-                const int wt = P.wtap[tap];
-                uint8_t* sb = st + A_BYTES * (SPLIT ? 2 : 1);
-                if (elect_one()) {
-                    mbar_expect_tx(bar_full + stage, (uint32_t)C::STAGE_BYTES);
-                    tma_load_4d(&P.a_hi[mi], st, bar_full + stage, c0, xx, yy, t.img);
-                    if (SPLIT) tma_load_4d(&P.a_lo[mi], st + A_BYTES, bar_full + stage, c0, xx, yy, t.img);
-                    tma_load_3d(&P.w_hi, sb, bar_full + stage, chunk * KCHUNK, t.n_idx * N_TILE, wt);
-                    if (SPLIT) tma_load_3d(&P.w_lo, sb + C::B_BYTES, bar_full + stage, chunk * KCHUNK, t.n_idx * N_TILE, wt);
+            for (int g = 0; g < P.ngroups; g++) {
+                const int first = P.g_first[g], cnt = P.g_cnt[g];
+                const int xx = t.x0 + P.dx[first], yy = t.y0 + P.dy[first];
+                for (int chunk = 0; chunk < nchunks; chunk++) {
+                    const bool second = chunk >= P.chunks0;
+                    const int mi = second ? 1 : P.tmap[first];
+                    const int c0 = (second ? chunk - P.chunks0 : chunk) * KCHUNK;
+                    // one box of a_rows image rows serves every tap of the group
+                    mbar_wait(a_empty + as, aph ^ 1);
+                    uint8_t* sa = smem + as * a_stage_bytes;
+                    if (elect_one()) {
+                        mbar_expect_tx(a_full + as, (uint32_t)a_stage_bytes);
+                        tma_load_4d(&P.a_hi[mi], sa, a_full + as, c0, xx, yy, t.img);
+                        if (SPLIT) tma_load_4d(&P.a_lo[mi], sa + a_op_bytes, a_full + as, c0, xx, yy, t.img);
+                    }
+                    __syncwarp();
+                    if (++as == P.a_stages) { as = 0; aph ^= 1; }
+                    for (int i = 0; i < cnt; i++) {
+                        mbar_wait(b_empty + bs, bph ^ 1);
+                        uint8_t* sb = b_ring + bs * C::B_STAGE_BYTES;
+                        const int wt = P.wtap[first + i];
+                        if (elect_one()) {
+                            mbar_expect_tx(b_full + bs, (uint32_t)C::B_STAGE_BYTES);
+                            tma_load_3d(&P.w_hi, sb, b_full + bs, chunk * KCHUNK, t.n_idx * N_TILE, wt);
+                            if (SPLIT) tma_load_3d(&P.w_lo, sb + C::B_BYTES, b_full + bs, chunk * KCHUNK, t.n_idx * N_TILE, wt);
+                        }
+                        __syncwarp();
+                        if (++bs == P.b_stages) { bs = 0; bph ^= 1; }
+                    }
                 }
-                __syncwarp();
-                if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
             }
         }
     } else if (warp < NUM_CONSUMERS / 32) {
         // ================================ consumers (2 warpgroups, 64 tile rows each) ==================
         const uint32_t smem_base = smem_u32(smem);
-        const uint32_t a_row0 = (uint32_t)(warp >> 2) * 64u * 128u;
+        const uint32_t b_base = smem_u32(b_ring);
+        const uint32_t a_row0 = (uint32_t)(warp >> 2) * 8u * ROW_BYTES;      // tile rows 8 g .. 8 g + 7
         // The e4m3 products get their own accumulator: Hopper's fp8 wgmma adds into D with a reduced-precision
         // accumulation, which would truncate the fp16 main product's fp32 sum.  The two are added in the epilogue.
         float acc[N_TILE / 2];
         float acc8[MODE == MODE_F8 ? N_TILE / 2 : 1];
-        int stage = 0; uint32_t phase = 0;
+        int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
         for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
             const TileCoord t = decode_tile(P, tile, m_tiles);
 #pragma unroll
             for (int i = 0; i < N_TILE / 2; i++) acc[i] = 0.f;
 #pragma unroll
             for (int i = 0; i < (MODE == MODE_F8 ? N_TILE / 2 : 1); i++) acc8[i] = 0.f;
-            int prev = -1;
-            for (int s = 0; s < ksteps; s++) {
-                mbar_wait(bar_full + stage, phase);
-                const uint32_t a_hi = smem_base + stage * C::STAGE_BYTES + a_row0;
-                const uint32_t a_lo = a_hi + A_BYTES;
-                const uint32_t b_hi = smem_base + stage * C::STAGE_BYTES + A_BYTES * (SPLIT ? 2 : 1);
-                const uint32_t b_lo = b_hi + C::B_BYTES;
-                wgmma_fence();
+            // B entry of the last committed wgmma group, and the A entry whose last tap is in that group: both are
+            // released once the group has retired
+            int prev_b = -1, prev_a = -1;
+            for (int g = 0; g < P.ngroups; g++) {
+                const int cnt = P.g_cnt[g];
+                for (int chunk = 0; chunk < nchunks; chunk++) {
+                    mbar_wait(a_full + as, aph);
+                    const uint32_t a_hi = smem_base + as * a_stage_bytes + a_row0;
+                    for (int i = 0; i < cnt; i++) {
+                        mbar_wait(b_full + bs, bph);
+                        const uint32_t ai = a_hi + i * ROW_BYTES, al = ai + a_op_bytes;      // tap i: rows i .. i + 15
+                        const uint32_t b_hi = b_base + bs * C::B_STAGE_BYTES, b_lo = b_hi + C::B_BYTES;
+                        wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < KCHUNK / 16; k++) {
-                    const uint64_t da = make_desc(a_hi + k * 32), db = make_desc(b_hi + k * 32);
-                    wgmma_f16<N_TILE>(acc, da, db);
-                    if constexpr (MODE == MODE_F8) {
-                        wgmma_e4m3<N_TILE>(acc8, make_desc(a_lo + k * 32), make_desc(b_lo + k * 32));
-                    } else if constexpr (MODE == MODE_FP16X3) {
-                        wgmma_f16<N_TILE>(acc, da, make_desc(b_lo + k * 32));
-                        wgmma_f16<N_TILE>(acc, make_desc(a_lo + k * 32), db);
+                        for (int k = 0; k < KCHUNK / 16; k++) {
+                            const uint64_t da = make_desc(ai + k * 32), db = make_desc(b_hi + k * 32);
+                            wgmma_f16<N_TILE>(acc, da, db);
+                            if constexpr (MODE == MODE_F8) {
+                                wgmma_e4m3<N_TILE>(acc8, make_desc(al + k * 32), make_desc(b_lo + k * 32));
+                            } else if constexpr (MODE == MODE_FP16X3) {
+                                wgmma_f16<N_TILE>(acc, da, make_desc(b_lo + k * 32));
+                                wgmma_f16<N_TILE>(acc, make_desc(al + k * 32), db);
+                            }
+                        }
+                        wgmma_commit();
+                        // the previous wgmma group has retired: its entries may be refilled
+                        if (prev_b >= 0) {
+                            wgmma_wait<1>();
+                            if (lane == 0) {
+                                mbar_arrive(b_empty + prev_b);
+                                if (prev_a >= 0) mbar_arrive(a_empty + prev_a);
+                            }
+                            prev_a = -1;
+                        }
+                        prev_b = bs;
+                        if (++bs == P.b_stages) { bs = 0; bph ^= 1; }
                     }
+                    prev_a = as;
+                    if (++as == P.a_stages) { as = 0; aph ^= 1; }
                 }
-                wgmma_commit();
-                // the previous stage's wgmma group has retired: its shared memory may be refilled
-                if (prev >= 0) {
-                    wgmma_wait<1>();
-                    if (lane == 0) mbar_arrive(bar_empty + prev);
-                }
-                prev = stage;
-                if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
             }
             wgmma_wait<0>();
 #pragma unroll
@@ -546,7 +592,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
 #pragma unroll
                 for (int i = 0; i < N_TILE / 2; i++) { acc_fence(acc8[i]); acc[i] += acc8[i]; }
             }
-            if (lane == 0) mbar_arrive(bar_empty + prev);
+            if (lane == 0) { mbar_arrive(b_empty + prev_b); mbar_arrive(a_empty + prev_a); }
             if constexpr (FUSED) epilogue_fused<N_TILE>(P, acc, t, warp, lane, s_stats, s_ss);
             else                 epilogue_plain<N_TILE>(P, acc, t, warp, lane, s_stats);
         }
@@ -655,21 +701,63 @@ struct lwb_conv_plan {
     Launch launches[4];
 };
 
-// Plain NHWC activation map: dims [C, W, H, N].
-static int map_nhwc(CUtensorMap* m, const uint16_t* base, int n, int h, int w, int c)
+// Plain NHWC activation map: dims [C, W, H, N], boxes of `rows` image rows.
+static int map_nhwc(CUtensorMap* m, const uint16_t* base, int n, int h, int w, int c, int rows)
 {
     const uint64_t dims[4] = {(uint64_t)c, (uint64_t)w, (uint64_t)h, (uint64_t)n};
     const uint64_t str[3] = {(uint64_t)c * 2, (uint64_t)w * c * 2, (uint64_t)h * w * c * 2};
-    const uint32_t box[4] = {(uint32_t)KCHUNK, TILE_W, TILE_H, 1};
+    const uint32_t box[4] = {(uint32_t)KCHUNK, TILE_W, (uint32_t)rows, 1};
     return encode_map(m, base, 4, dims, str, box);
 }
 // Parity view (py, px) of an NHWC tensor for stride-2 convs: element (y', x') = input (2y'+py, 2x'+px).
-static int map_nhwc_parity(CUtensorMap* m, const uint16_t* base, int n, int h, int w, int c, int py, int px)
+static int map_nhwc_parity(CUtensorMap* m, const uint16_t* base, int n, int h, int w, int c, int py, int px, int rows)
 {
     const uint64_t dims[4] = {(uint64_t)c, (uint64_t)((w - px + 1) / 2), (uint64_t)((h - py + 1) / 2), (uint64_t)n};
     const uint64_t str[3] = {(uint64_t)2 * c * 2, (uint64_t)2 * w * c * 2, (uint64_t)h * w * c * 2};
-    const uint32_t box[4] = {(uint32_t)KCHUNK, TILE_W, TILE_H, 1};
+    const uint32_t box[4] = {(uint32_t)KCHUNK, TILE_W, (uint32_t)rows, 1};
     return encode_map(m, base + ((size_t)py * w + px) * c, 4, dims, str, box);
+}
+
+// Orders the taps of p into y-halo groups: taps that read the same input view (tmap) at the same dx with consecutive
+// ascending dy share one activation box (at most MAX_GROUP taps per group; a tap that matches nothing is a group of
+// one).  wtap keeps addressing the weights, so the order of the taps is free.  Sets the groups and a_rows.
+static void group_taps(ConvParams& p)
+{
+    int order[MAX_TAPS];
+    for (int t = 0; t < p.ntaps; t++) order[t] = t;
+    std::stable_sort(order, order + p.ntaps, [&](int a, int b) {
+        if (p.tmap[a] != p.tmap[b]) return p.tmap[a] < p.tmap[b];
+        if (p.dx[a] != p.dx[b]) return p.dx[a] < p.dx[b];
+        return p.dy[a] < p.dy[b];
+    });
+    const ConvParams src = p;
+    int longest = 0;
+    p.ngroups = 0;
+    for (int t = 0; t < p.ntaps; t++) {
+        const int o = order[t];
+        p.dy[t] = src.dy[o]; p.dx[t] = src.dx[o]; p.tmap[t] = src.tmap[o]; p.wtap[t] = src.wtap[o];
+        const bool joins = t > 0 && p.tmap[t] == p.tmap[t - 1] && p.dx[t] == p.dx[t - 1] && p.dy[t] == p.dy[t - 1] + 1 &&
+                           p.g_cnt[p.ngroups - 1] < MAX_GROUP;
+        if (!joins) { p.g_first[p.ngroups] = (signed char)t; p.g_cnt[p.ngroups] = 0; p.ngroups++; }
+        p.g_cnt[p.ngroups - 1]++;
+        longest = std::max(longest, (int)p.g_cnt[p.ngroups - 1]);
+    }
+    p.a_rows = TILE_H + longest - 1;
+}
+
+// Ring depths inside RING_BYTES: at least two entries per ring (the consumers release an entry one wgmma group late),
+// otherwise the split that keeps the most taps in flight, min(A entries x longest group, B entries).
+static void pick_rings(ConvParams& p, int n_tile, bool split)
+{
+    const int ops = split ? 2 : 1;
+    const int a_bytes = p.a_rows * ROW_BYTES * ops, b_bytes = n_tile * 128 * ops;
+    const int longest = p.a_rows - TILE_H + 1;
+    int best = 0;
+    for (int a = 2; a <= MAX_STAGES; a++) {
+        const int b = std::min(MAX_STAGES, (RING_BYTES - a * a_bytes) / b_bytes);
+        if (b < 2) break;
+        if (std::min(a * longest, b) > best) { best = std::min(a * longest, b); p.a_stages = a; p.b_stages = b; }
+    }
 }
 
 extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
@@ -690,7 +778,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     int n_tile = pick_n_tile(d->cout, d->n_tile);
     LWB_CHECK_ARG(n_tile > 0 && d->cout % n_tile == 0, "no N tile divides cout");
     if (d->halo) {
-        // halo plans ("same"-padded stride-1 k x k convs and the row-K stem) run through the per-tap kernel below
+        // halo plans ("same"-padded stride-1 k x k convs and the row-K stem) run through the tap-group kernel below
         LWB_CHECK_ARG(d->stride == 1 && !d->transposed && d->dil == 1, "halo mode needs stride 1, dilation 1, not transposed");
         if (d->rowk) LWB_CHECK_ARG(d->kw <= 8 && d->cin0 == 8 && d->cin1 == 0 && d->row_pitch >= d->w_in + 8, "row-K shape");
         else         LWB_CHECK_ARG(d->kw <= 9 && (d->kw & 1) && (d->kh & 1), "halo mode needs an odd kernel, kw <= 9, with 'same' padding (kh/2, kw/2)");
@@ -713,6 +801,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         p.stats = stats;
         p.out_scale = f8 ? ldexpf(1.f, -d->w_exp) : 1.f;      // weights are packed x 2^w_exp in f8 mode (lwb_pack_conv_weight_f8)
         L.n_tile = n_tile; L.mode = d->split; L.fused = false;
+        pick_rings(p, n_tile, split);
         const long total = (long)p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
         L.grid = (int)(total < sms ? total : sms);
     };
@@ -725,10 +814,13 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         LWB_CHECK_ARG(d->h_out == d->h_in && d->w_out == d->w_in && d->row_pitch >= d->w_in + 8, "row-K shape");
         Launch& L = plan->launches[plan->num++];
         memset(&L.p, 0, sizeof(L.p));
+        L.p.ntaps = d->kh; L.p.chunks0 = 1; L.p.chunks1 = 0;
+        for (int ky = 0; ky < d->kh; ky++) { L.p.dy[ky] = (signed char)ky; L.p.dx[ky] = 0; L.p.tmap[ky] = 0; L.p.wtap[ky] = (short)ky; }
+        group_taps(L.p);
         const int hp = d->h_in + d->kh - 1;
         const uint64_t dims[4] = {64, (uint64_t)d->w_in, (uint64_t)hp, (uint64_t)d->n};
         const uint64_t str[3] = {16, (uint64_t)d->row_pitch * 16, (uint64_t)hp * d->row_pitch * 16};
-        const uint32_t box[4] = {KCHUNK, TILE_W, TILE_H, 1};
+        const uint32_t box[4] = {KCHUNK, TILE_W, (uint32_t)L.p.a_rows, 1};
         if ((rc = encode_map(&L.p.a_hi[0], x0_hi, 4, dims, str, box)) != LWB_OK) return fail(rc);
         if (split && (rc = encode_map(&L.p.a_lo[0], x0_lo, 4, dims, str, box)) != LWB_OK) return fail(rc);
         const uint64_t wd[3] = {64, (uint64_t)d->cout, (uint64_t)d->kh};
@@ -736,8 +828,6 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         const uint32_t wb[3] = {KCHUNK, (uint32_t)n_tile, 1};
         if ((rc = encode_map(&L.p.w_hi, w_hi, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
         if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
-        L.p.ntaps = d->kh; L.p.chunks0 = 1; L.p.chunks1 = 0;
-        for (int ky = 0; ky < d->kh; ky++) { L.p.dy[ky] = (signed char)ky; L.p.dx[ky] = 0; L.p.tmap[ky] = 0; L.p.wtap[ky] = (short)ky; }
         L.p.oy_mul = 1; L.p.ox_mul = 1; L.p.oy_add = 0; L.p.ox_add = 0;
         finish(L, d->h_out, d->w_out);
         *plan_out = plan;
@@ -764,15 +854,16 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         LWB_CHECK_ARG(d->cout % 32 == 0 && ncols % n_tile == 0, "merged transposed conv needs cout in multiples of 32");
         Launch& L = plan->launches[plan->num++];
         memset(&L.p, 0, sizeof(L.p));
-        if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0)) != LWB_OK) return fail(rc);
-        if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0)) != LWB_OK) return fail(rc);
+        for (int t = 0; t < 4; t++) { L.p.dy[t] = (signed char)(t >> 1); L.p.dx[t] = (signed char)(t & 1); L.p.tmap[t] = 0; L.p.wtap[t] = (short)t; }
+        L.p.ntaps = 4; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = 0;
+        group_taps(L.p);
+        if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
+        if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
         const uint64_t mwd[3] = {(uint64_t)cin_total, (uint64_t)ncols, 4};
         const uint64_t mws[2] = {(uint64_t)cin_total * 2, (uint64_t)ncols * cin_total * 2};
         const uint32_t mwb[3] = {(uint32_t)KCHUNK, (uint32_t)n_tile, 1};
         if ((rc = encode_map(&L.p.w_hi, w_hi, 3, mwd, mws, mwb)) != LWB_OK) return fail(rc);
         if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, mwd, mws, mwb)) != LWB_OK) return fail(rc);
-        for (int t = 0; t < 4; t++) { L.p.dy[t] = (signed char)(t >> 1); L.p.dx[t] = (signed char)(t & 1); L.p.tmap[t] = 0; L.p.wtap[t] = (short)t; }
-        L.p.ntaps = 4; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = 0;
         L.p.oy_mul = 2; L.p.ox_mul = 2; L.p.oy_add = 0; L.p.ox_add = 0;
         finish(L, d->h_in, d->w_in);
         L.p.phase_cols = d->cout;
@@ -791,10 +882,6 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         for (int a = 0; a < 2; a++) for (int b = 0; b < 2; b++) {
             Launch& L = plan->launches[plan->num++];
             memset(&L.p, 0, sizeof(L.p));
-            if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0)) != LWB_OK) return fail(rc);
-            if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0)) != LWB_OK) return fail(rc);
-            if ((rc = encode_map(&L.p.w_hi, w_hi, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
-            if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
             const int ky_list[2][2] = {{1, -1}, {2, 0}}, d_list[2][2] = {{0, 0}, {0, 1}}, cnt[2] = {1, 2};
             int t = 0;
             for (int i = 0; i < cnt[a]; i++) for (int j = 0; j < cnt[b]; j++) {
@@ -803,6 +890,11 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
                 t++;
             }
             L.p.ntaps = t; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = 0;
+            group_taps(L.p);
+            if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
+            if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
+            if ((rc = encode_map(&L.p.w_hi, w_hi, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
+            if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
             L.p.oy_mul = 2; L.p.ox_mul = 2; L.p.oy_add = a; L.p.ox_add = b;
             finish(L, d->h_in, d->w_in);
         }
@@ -831,17 +923,19 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     }
     L.p.ntaps = t; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = d->cin1 / KCHUNK;
     L.p.oy_mul = 1; L.p.ox_mul = 1; L.p.oy_add = 0; L.p.ox_add = 0;
+    group_taps(L.p);
+    const int rows = L.p.a_rows;
     if (d->stride == 1) {
-        if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0)) != LWB_OK) return fail(rc);
-        if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0)) != LWB_OK) return fail(rc);
+        if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, rows)) != LWB_OK) return fail(rc);
+        if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0, rows)) != LWB_OK) return fail(rc);
         if (d->cin1) {
-            if ((rc = map_nhwc(&L.p.a_hi[1], x1_hi, d->n, d->h_in, d->w_in, d->cin1)) != LWB_OK) return fail(rc);
-            if (split && (rc = map_nhwc(&L.p.a_lo[1], x1_lo, d->n, d->h_in, d->w_in, d->cin1)) != LWB_OK) return fail(rc);
+            if ((rc = map_nhwc(&L.p.a_hi[1], x1_hi, d->n, d->h_in, d->w_in, d->cin1, rows)) != LWB_OK) return fail(rc);
+            if (split && (rc = map_nhwc(&L.p.a_lo[1], x1_lo, d->n, d->h_in, d->w_in, d->cin1, rows)) != LWB_OK) return fail(rc);
         }
     } else {
         for (int py = 0; py < 2; py++) for (int px = 0; px < 2; px++) {
-            if ((rc = map_nhwc_parity(&L.p.a_hi[py * 2 + px], x0_hi, d->n, d->h_in, d->w_in, d->cin0, py, px)) != LWB_OK) return fail(rc);
-            if (split && (rc = map_nhwc_parity(&L.p.a_lo[py * 2 + px], x0_lo, d->n, d->h_in, d->w_in, d->cin0, py, px)) != LWB_OK) return fail(rc);
+            if ((rc = map_nhwc_parity(&L.p.a_hi[py * 2 + px], x0_hi, d->n, d->h_in, d->w_in, d->cin0, py, px, rows)) != LWB_OK) return fail(rc);
+            if (split && (rc = map_nhwc_parity(&L.p.a_lo[py * 2 + px], x0_lo, d->n, d->h_in, d->w_in, d->cin0, py, px, rows)) != LWB_OK) return fail(rc);
         }
     }
     if ((rc = encode_map(&L.p.w_hi, w_hi, 3, wd, ws, wb)) != LWB_OK) return fail(rc);

@@ -138,7 +138,7 @@ def _align_corners():
 
 def _halo_mode():
     """LWB_HALO: '0' (default) = CUDA-core 7x7 heads; 'auto' = halo plans for the row-K stem and the skippers + 7x7
-    heads on tensor cores (N tile 16); 'all' = also the residual blocks.  Halo plans run through the same per-tap conv
+    heads on tensor cores (N tile 16); 'all' = also the residual blocks.  Halo plans run through the same tap-group conv
     kernel as the others."""
     if precision_mode() == "fp16f8":
         return '0'                                         # halo plans have no fp8 path

@@ -141,7 +141,7 @@ typedef struct lwb_conv_desc {
     int row_pitch;            /* rowk: pixels per padded row (>= w_in + 8) */
     int n_tile;               /* 0 = auto; else force the N tile (16/32/64/128, must divide cout; 256 runs as 128) */
     int halo;                 /* 1 = halo plan (stride-1 'same' k x k convs and the row-K stem): checked as such, then run
-                                 by the same per-tap kernel as halo = 0 */
+                                 by the same tap-group kernel as halo = 0 */
     int w_exp;                /* split = 2: the power of two the weights were packed with (lwb_pack_conv_weight_f8) */
     int pad_w;                /* horizontal padding when it differs from pad (e.g. a 7x1 filter); -1 = same as pad */
 } lwb_conv_desc;

@@ -1,27 +1,148 @@
-"""Micro-benchmark of single conv layers of the wgmma engine (CUDA events): operand mode, N tile."""
+"""Micro-benchmark of single conv layers of the wgmma engine (CUDA events), run from the repository root on a GPU.
+
+The layers are the ones the flagship step runs (256x256, 16 frames as two sub-batch streams of 8), each in the three
+operand modes: fp16f8 (the default, split=2), fp16x3 (split=1) and single-pass fp16 (split=0).  The row-K stem has no
+fp8 path and runs fp16x3 where fp16f8 is asked for, as in the generator.  Beside the time, every layer prints the
+operand bytes per algorithmic FLOP that the TMA unit moves from L2 into shared memory: once for a schedule that fetches
+a 16-row activation tile per filter tap ("per-tap") and once for the y-halo tap groups the engine runs ("grouped").
+
+    python tools/conv_microbench.py [--batch 8] [--reps 50] [--only res] [--json out.json]
+"""
+import argparse
+import json
 import sys
+
 import torch
+
 sys.path.insert(0, ".")
-from impersonator_b200 import kernels as K
+from impersonator_b200 import kernels as K  # noqa: E402
+from impersonator_b200.generator import merge_transposed_weight  # noqa: E402
 
-dev = torch.device("cuda")
-torch.manual_seed(0)
+TILE_H, TILE_W, KCHUNK, MAX_GROUP = 16, 8, 64, 8
+MODES = (("fp16f8", 2), ("fp16x3", 1), ("fp16", 0))
 
 
-def bench(name, n, cin, cout, h, k, stats=True, halo=False, n_tile=0, split=True, rowk=False, cin1=0, reps=20):
-    if rowk:
-        x = (torch.randn(n, h + 6, h + 8, 8, device=dev).half(), torch.randn(n, h + 6, h + 8, 8, device=dev).half())
-        w = (torch.randn(7, cout, 64, device=dev).half(), torch.randn(7, cout, 64, device=dev).half())
-        d = K.make_conv_desc(n, h, h, 8, cout, 7, 7, stride=1, pad=3, split=split, rowk=True, row_pitch=h + 8, halo=halo, n_tile=n_tile)
-        x1 = None
+def tap_groups(taps):
+    """(view, dy, dx) per tap -> (groups, largest group): taps sharing view and dx with consecutive dy form one group
+    (the rule of lwb_conv_plan_create)."""
+    groups, run, prev = 0, 0, None
+    longest = 0
+    for v, dy, dx in sorted(taps, key=lambda t: (t[0], t[2], t[1])):
+        if prev is not None and (v, dx) == (prev[0], prev[2]) and dy == prev[1] + 1 and run < MAX_GROUP:
+            run += 1
+        else:
+            groups, run = groups + 1, 1
+        longest = max(longest, run)
+        prev = (v, dy, dx)
+    return groups, longest
+
+
+def launch_taps(spec):
+    """Per launch of the plan: the (view, dy, dx) list of its taps."""
+    kind, k = spec["kind"], spec.get("k", 3)
+    if kind == "rowk":
+        return [[(0, ky, 0) for ky in range(7)]]
+    if kind == "merged":
+        return [[(0, t >> 1, t & 1) for t in range(4)]]
+    if kind == "transposed":
+        d = ([0], [0, 1])
+        return [[(0, dy, dx) for dy in d[a] for dx in d[b]] for a in range(2) for b in range(2)]
+    kh, kw = (k, 1) if kind == "heads" else (k, k)
+    pad, pad_w = k // 2, (0 if kind == "heads" else k // 2)
+    taps = []
+    for ky in range(kh):
+        for kx in range(kw):
+            oy, ox = ky - pad, kx - pad_w
+            if spec.get("stride", 1) == 2:
+                py, px = oy % 2, ox % 2
+                taps.append((2 * py + px, (oy - py) // 2, (ox - px) // 2))
+            else:
+                taps.append((0, oy, ox))
+    return [taps]
+
+
+def operand_bytes(spec, n, n_tile, split, grouped):
+    """TMA bytes of the whole layer (A hi/lo + B hi/lo, every tile)."""
+    ops = 2 if split else 1
+    chunks = 1 if spec["kind"] == "rowk" else (spec["cin"] + spec.get("cin1", 0)) // KCHUNK
+    dom = spec["h"] // 2 if spec.get("stride", 1) == 2 else spec["h"]
+    ncols = 4 * spec["cout"] if spec["kind"] == "merged" else spec["cout"]
+    tiles = n * -(-dom // TILE_H) * -(-dom // TILE_W) * (ncols // n_tile)
+    total = 0
+    for taps in launch_taps(spec):
+        if grouped:
+            groups, longest = tap_groups(taps)
+            a_rows = groups * (TILE_H + longest - 1)
+        else:
+            a_rows = len(taps) * TILE_H
+        total += tiles * chunks * ops * (a_rows * TILE_W * 128 + len(taps) * n_tile * 128)
+    return total
+
+
+def make_plan(spec, n, split, dev):
+    kind, h, cin, cout = spec["kind"], spec["h"], spec.get("cin", 8), spec["cout"]
+    cin1 = spec.get("cin1", 0)
+    x1 = None
+    lo = lambda t: (t * 1e-3).half()                                # noqa: E731  (any bits: timing only)
+    if kind == "rowk":
+        split = min(split, 1)
+        xs = torch.randn(n, h + 6, h + 8, 8, device=dev)
+        x = (xs.half(), lo(xs))
+        wt = torch.randn(cout, 6, 7, 7, device=dev) * 0.05
+        w = K.pack_conv_weight_rowk(wt, split=split)
+        d = K.make_conv_desc(n, h, h, 8, cout, 7, 7, stride=1, pad=3, split=split, rowk=True, row_pitch=h + 8)
+        out_hw = h
     else:
-        x = (torch.randn(n, h, h, cin, device=dev).half(), torch.randn(n, h, h, cin, device=dev).half())
-        x1 = (torch.randn(n, h, h, cin1, device=dev).half(), torch.randn(n, h, h, cin1, device=dev).half()) if cin1 else None
-        w = (torch.randn(k * k, cout, cin + cin1, device=dev).half(), torch.randn(k * k, cout, cin + cin1, device=dev).half())
-        d = K.make_conv_desc(n, h, h, cin, cout, k, k, stride=1, pad=k // 2, cin1=cin1, split=split, halo=halo, n_tile=n_tile)
-    out = torch.empty((n, h, h, cout), device=dev)
-    st = torch.zeros((n, cout, 2), dtype=torch.float64, device=dev) if stats else None
-    plan = K.ConvPlan(d, x, x1, w, out, st)
+        xs = torch.randn(n, h, h, cin, device=dev)
+        x = (xs.half(), lo(xs))
+        if cin1:
+            x1s = torch.randn(n, h, h, cin1, device=dev)
+            x1 = (x1s.half(), lo(x1s))
+        k = spec.get("k", 3)
+        if kind in ("transposed", "merged"):
+            wt = torch.randn(cin, cout, 3, 3, device=dev) * 0.05
+            if kind == "merged":
+                w = K.pack_conv_weight(merge_transposed_weight(wt), split=split)
+            else:
+                w = K.pack_conv_weight(wt, transposed=True, split=split)
+            d = K.make_conv_desc(n, h, h, cin, cout, 3, 3, stride=2, pad=1, transposed=True, split=split)
+            if kind == "merged":
+                d.transposed = 2
+            out_hw = 2 * h
+        elif kind == "heads":
+            wt = torch.randn(cout, cin, k, 1, device=dev) * 0.05
+            w = K.pack_conv_weight(wt, split=split)
+            d = K.make_conv_desc(n, h, h, cin, cout, k, 1, pad=k // 2, pad_w=0, split=split, n_tile=spec["n_tile"])
+            out_hw = h
+        else:
+            stride = spec.get("stride", 1)
+            wt = torch.randn(cout, cin + cin1, k, k, device=dev) * 0.05
+            w = K.pack_conv_weight(wt, split=split)
+            d = K.make_conv_desc(n, h, h, cin, cout, k, k, stride=stride, pad=k // 2, cin1=cin1, split=split)
+            out_hw = d.h_out
+    out = torch.empty((n, out_hw, out_hw, cout), device=dev)
+    st = torch.zeros((n, cout, 2), dtype=torch.float64, device=dev)
+    return K.ConvPlan(d, x, x1, w, out, st), split
+
+
+# the flagship's conv layers per sub-batch stream (ImpersonatorGenerator, 256x256, repeat_num 6, n_down 3)
+LAYERS = [
+    ("stem R7x7 8->64 @256", dict(kind="rowk", h=256, cout=64)),
+    ("enc C3x3s2 64->128 @256", dict(kind="conv", stride=2, h=256, cin=64, cout=128)),
+    ("enc C3x3s2 128->256 @128", dict(kind="conv", stride=2, h=128, cin=128, cout=256)),
+    ("enc C3x3s2 256->512 @64", dict(kind="conv", stride=2, h=64, cin=256, cout=512)),
+    ("res C3x3 512->512 @32 (x12)", dict(kind="conv", h=32, cin=512, cout=512)),
+    ("dec T3x3 512->256 @32 (4 phases)", dict(kind="transposed", h=32, cin=512, cout=256)),
+    ("skip C3x3 256+256->256 @64", dict(kind="conv", h=64, cin=256, cin1=256, cout=256)),
+    ("dec T3x3 256->128 @64 (merged)", dict(kind="merged", h=64, cin=256, cout=128)),
+    ("skip C3x3 128+128->128 @128", dict(kind="conv", h=128, cin=128, cin1=128, cout=128)),
+    ("dec T3x3 128->64 @128 (merged)", dict(kind="merged", h=128, cin=128, cout=64)),
+    ("skip C3x3 64+64->64 @256", dict(kind="conv", h=256, cin=64, cin1=64, cout=64)),
+    ("heads C7x1 64->28 @256 (N 32)", dict(kind="heads", k=7, h=256, cin=64, cout=32, n_tile=32)),
+]
+
+
+def time_plan(plan, reps):
     for _ in range(3):
         plan.run()
     torch.cuda.synchronize()
@@ -31,15 +152,41 @@ def bench(name, n, cin, cout, h, k, stats=True, halo=False, n_tile=0, split=True
         plan.run()
     e1.record()
     torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / reps
-    print("%-44s stats=%d halo=%d ntile=%3d : %7.3f ms  %7.1f TF/s algorithmic" % (name, stats, halo, n_tile or -1, ms, plan.flops / ms / 1e9))
+    return e0.elapsed_time(e1) / reps
 
 
-bench("stem rowk 8->64 @256 B16", 16, 8, 64, 256, 7, rowk=True)
-bench("skipper 64+64->64 @256 B16", 16, 64, 64, 256, 3, cin1=64)
-bench("skipper 128+128->128 @128 B16", 16, 128, 128, 128, 3, cin1=128)
-bench("res 512->512 @32 B16", 16, 512, 512, 32, 3)
-bench("res 512->512 @32 B16 fast", 16, 512, 512, 32, 3, split=False)
-bench("res 512->512 @32 B16 n64", 16, 512, 512, 32, 3, n_tile=64)
-bench("skipper 64+64->64 @256 B16 fast", 16, 64, 64, 256, 3, cin1=64, split=False)
-bench("stem rowk 8->64 @256 B16 fast", 16, 8, 64, 256, 7, rowk=True, split=False)
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("--batch", type=int, default=8)
+    ap.add_argument("--reps", type=int, default=50)
+    ap.add_argument("--only", default="", help="substring filter on the layer name")
+    ap.add_argument("--json", default="", help="also write the rows to this file")
+    a = ap.parse_args()
+    dev = torch.device("cuda")
+    torch.manual_seed(0)
+    torch.set_grad_enabled(False)
+    rows = []
+    print("%-34s %-7s %9s %9s %10s %10s" % ("layer (batch %d)" % a.batch, "mode", "ms", "TFLOP/s", "B/FLOP tap", "B/FLOP grp"))
+    for name, spec in LAYERS:
+        if a.only and a.only not in name:
+            continue
+        for mode, split in MODES:
+            plan, ran = make_plan(spec, a.batch, split, dev)
+            ms = time_plan(plan, a.reps)
+            n_tile = spec.get("n_tile") or (128 if (4 * spec["cout"] if spec["kind"] == "merged" else spec["cout"]) % 128 == 0 else 64)
+            bpf = [operand_bytes(spec, a.batch, n_tile, ran, g) / plan.flops for g in (False, True)]
+            row = dict(layer=name, mode=mode, ran_split=ran, ms=ms, tflops=plan.flops / ms / 1e9,
+                       bytes_per_flop_per_tap=bpf[0], bytes_per_flop_grouped=bpf[1])
+            rows.append(row)
+            print("%-34s %-7s %9.4f %9.1f %10.4f %10.4f" % (name, mode + ("*" if ran != split else ""), ms, row["tflops"], bpf[0], bpf[1]))
+            del plan
+    print("* the row-K stem has no fp8 path: fp16x3 operands")
+    props = torch.cuda.get_device_properties(0)
+    print("device: %s" % props.name)
+    if a.json:
+        with open(a.json, "w") as f:
+            json.dump(dict(device=props.name, batch=a.batch, reps=a.reps, rows=rows), f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
