@@ -20,6 +20,13 @@
 // phase lives in address bits 7-9 and does not change).  The K loop runs (group, chunk, tap in group):
 // one A fetch per (group, chunk) into the A ring, one weight fetch per tap into the B ring.
 //
+// Swapped orientation (SWAP, every plan whose N tile is 64): the same 16K-output accumulator budget is spent as 64 output
+// channels x 256 pixels (32 x 8), with the channels on the wgmma M side: D^T[cout, pixel] = W[cout, K] . X[pixel, K]^T.
+// The [64][128 B] weight tile is the A operand and the activation box the B operand (both already K-major SWIZZLE_128B);
+// consumer warpgroup g issues M64 x N128 wgmmas on box rows 16 g .. 16 g + 15 (+ the tap's row offset).  Against an
+// N = 64 tile of 128 pixels this halves the weight fetches per FLOP and the per-tile overheads, and the wider wgmma reads
+// less shared memory per tensor-core cycle.
+//
 // Precision: x ~= x_hi + x_lo, w ~= w_hi + w_lo in fp16; with SPLIT the accumulator receives
 // x_hi*w_hi + x_hi*w_lo + x_lo*w_hi (fp32 accumulate), which reproduces the fp32 reference
 // convolution to ~1e-5 (single pass fp16 cannot meet the 1e-3 parity bar, SURVEY.md 0.4).
@@ -53,10 +60,12 @@
 namespace {
 
 constexpr int TILE_H = 16, TILE_W = 8;          // output pixels per tile (M = 128)
+constexpr int SWAP_N_TILE = 64;                  // plans with this N tile run the swapped orientation ...
+constexpr int SWAP_TILE_H = 32;                  // ... on 32 x 8 = 256-pixel tiles
 constexpr int KCHUNK = 64;                       // fp16 elements per K stage (128 B swizzle span)
 constexpr int ROW_BYTES = TILE_W * 128;          // one image row of an A box = one SWIZZLE_128B atom
 constexpr int MAX_TAPS = 49;
-constexpr int MAX_GROUP = 8;                     // taps per y-halo group: A boxes of at most TILE_H + 7 rows
+constexpr int MAX_GROUP = 8;                     // taps per y-halo group: A boxes of at most tile height + 7 rows
 constexpr int RING_BYTES = 200 * 1024;           // A ring + B ring
 constexpr int MAX_STAGES = 8;                    // entries per ring
 constexpr int NUM_CONSUMERS = 256;               // warps 0..7: two consumer warpgroups
@@ -64,6 +73,11 @@ constexpr int NUM_THREADS = NUM_CONSUMERS + 32;  // warp 8: TMA producer
 constexpr int MAX_N_TILE = 128;                  // 64 fp32 accumulator registers per consumer thread
 static_assert(2 * 2 * (TILE_H + MAX_GROUP - 1) * ROW_BYTES + 2 * 2 * MAX_N_TILE * 128 <= RING_BYTES,
               "every plan needs two A and two B entries in the ring");
+static_assert(2 * 2 * (SWAP_TILE_H + MAX_GROUP - 1) * ROW_BYTES + 2 * 2 * SWAP_N_TILE * 128 <= RING_BYTES,
+              "every swapped plan needs two A and two B entries in the ring");
+static_assert(SWAP_N_TILE * (SWAP_TILE_H * TILE_W) == MAX_N_TILE * (TILE_H * TILE_W), "same accumulator budget");
+
+__host__ __device__ constexpr int tile_rows(int n_tile) { return n_tile == SWAP_N_TILE ? SWAP_TILE_H : TILE_H; }
 
 // InstanceNorm (+ReLU, +residual, +LWB warp-add) fused into the conv epilogue (k_conv_wg<.., FUSED = true>): the operands
 // of the NEXT layer leave the kernel directly, no fp32 raw tensor and no second pass over HBM.  See epilogue_fused.
@@ -91,7 +105,7 @@ struct ConvParams {
     short wtap[MAX_TAPS];
     int ngroups;                      // y-halo groups: taps g_first .. g_first + g_cnt - 1, dy consecutive (group_taps)
     signed char g_first[MAX_TAPS], g_cnt[MAX_TAPS];
-    int a_rows;                       // A box height: TILE_H + longest group - 1
+    int a_rows;                       // A box height: tile height + longest group - 1
     int a_stages, b_stages;           // ring depths inside RING_BYTES (pick_rings)
     float* out; int out_h, out_w, cout;
     int oy_mul, oy_add, ox_mul, ox_add;
@@ -191,12 +205,6 @@ template <> __device__ __forceinline__ void wgmma_f16<32>(float* d, uint64_t da,
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                  : "l"(da), "l"(db), "r"(1));
 }
-template <> __device__ __forceinline__ void wgmma_f16<64>(float* d, uint64_t da, uint64_t db) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-                 : "l"(da), "l"(db), "r"(1));
-}
 template <> __device__ __forceinline__ void wgmma_f16<128>(float* d, uint64_t da, uint64_t db) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
@@ -215,12 +223,6 @@ template <> __device__ __forceinline__ void wgmma_e4m3<32>(float* d, uint64_t da
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                  : "l"(da), "l"(db), "r"(1));
 }
-template <> __device__ __forceinline__ void wgmma_e4m3<64>(float* d, uint64_t da, uint64_t db) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-                 : "l"(da), "l"(db), "r"(1));
-}
 template <> __device__ __forceinline__ void wgmma_e4m3<128>(float* d, uint64_t da, uint64_t db) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
@@ -235,13 +237,14 @@ __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;
 struct TileCoord {
     int n_idx, img, y0, x0;
 };
+template <int TH>
 __device__ __forceinline__ TileCoord decode_tile(const ConvParams& P, int tile, int m_tiles) {
     TileCoord t;
     t.n_idx = tile / m_tiles;
     const int m_idx = tile % m_tiles;
     t.img = m_idx / (P.tiles_y * P.tiles_x);
     const int rem = m_idx % (P.tiles_y * P.tiles_x);
-    t.y0 = (rem / P.tiles_x) * TILE_H; t.x0 = (rem % P.tiles_x) * TILE_W;
+    t.y0 = (rem / P.tiles_x) * TH; t.x0 = (rem % P.tiles_x) * TILE_W;
     return t;
 }
 
@@ -267,15 +270,16 @@ __device__ __forceinline__ void warp_tile_stats(const float* acc, bool v0, bool 
     }
 }
 
-// s_stats of the 8 consumer warps -> one f64 atomic pair per column of the tile (all consumer threads).
-template <int N_TILE>
+// s_stats of the PARTS partial rows (8 consumer warps, or 2 warpgroups when swapped) -> one f64 atomic pair per column
+// of the tile (all consumer threads).
+template <int N_TILE, int PARTS = 8>
 __device__ __forceinline__ void flush_tile_stats(const ConvParams& P, const float2* s_stats, int img, int n_idx)
 {
     consumer_sync();
     for (int col = threadIdx.x; col < N_TILE; col += NUM_CONSUMERS) {
         float s = 0.f, q = 0.f;
 #pragma unroll
-        for (int w = 0; w < 8; w++) { const float2 v = s_stats[w * N_TILE + col]; s += v.x; q += v.y; }
+        for (int w = 0; w < PARTS; w++) { const float2 v = s_stats[w * N_TILE + col]; s += v.x; q += v.y; }
         int ch = n_idx * N_TILE + col;
         if (P.phase_cols > 0) ch %= P.phase_cols;      // the four phases of a channel share its statistics
         double* dst = P.stats + 2 * ((size_t)img * P.cout + ch);
@@ -320,6 +324,68 @@ __device__ __forceinline__ void epilogue_plain(const ConvParams& P, float* acc, 
     if (P.stats) {
         warp_tile_stats<N_TILE>(acc, valid[0], valid[1], warp, lane, s_stats);
         flush_tile_stats<N_TILE>(P, s_stats, t.img, t.n_idx);
+    }
+}
+
+// Epilogue of the swapped orientation: the accumulator is D^T, d[4j + 2h + e] = channel 16(warp%4) + lane/4 + 8h of the
+// N tile at pixel (tile row 16(warp/4) + j, column 2(lane%4) + e).  fp32 NHWC stores: one warp-wide store covers
+// 4 pixels x 8 consecutive channels, whole 32-byte sectors.  Channel statistics: in-thread over the valid pixels, the
+// quad (lanes of one channel) by shuffles, the two warpgroups through s_stats.
+__device__ __forceinline__ void epilogue_swapped(const ConvParams& P, float* acc, const TileCoord& t, int warp, unsigned lane,
+                                                 float2* s_stats)
+{
+    constexpr int N = SWAP_N_TILE;
+    const int wg = warp >> 2;
+    const int c0 = 16 * (warp & 3) + (int)(lane >> 2);                // channels c0 and c0 + 8 of the N tile
+    const int y0 = t.y0 + 16 * wg, x0 = t.x0 + 2 * (int)(lane & 3);
+    const int rows = P.dom_h - y0;                                     // row j is in the domain iff j < rows
+    const bool vx[2] = {x0 < P.dom_w, x0 + 1 < P.dom_w};
+    if (P.out_scale != 1.f) {
+#pragma unroll
+        for (int i = 0; i < 64; i++) acc[i] *= P.out_scale;
+    }
+    if (P.out) {
+        float* obase = P.out + (size_t)t.n_idx * N + c0;
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            if (j >= rows) break;
+            const size_t orow = ((size_t)t.img * P.out_h + (P.oy_mul * (y0 + j) + P.oy_add)) * P.out_w;
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                if (!vx[e]) continue;
+                float* o = obase + (orow + (P.ox_mul * (x0 + e) + P.ox_add)) * P.cout;
+                o[0] = acc[4 * j + e];
+                o[8] = acc[4 * j + 2 + e];
+            }
+        }
+    }
+    if (P.stats) {
+        float s[2] = {0.f, 0.f}, q[2] = {0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const bool v = j < rows && vx[e];
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const float a = v ? acc[4 * j + 2 * h + e] : 0.f;
+                    s[h] += a; q[h] += a * a;
+                }
+            }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+#pragma unroll
+            for (int off = 1; off <= 2; off <<= 1) {
+                s[h] += __shfl_xor_sync(0xffffffffu, s[h], off);
+                q[h] += __shfl_xor_sync(0xffffffffu, q[h], off);
+            }
+        }
+        if ((lane & 3) == 0) {
+            s_stats[wg * N + c0] = make_float2(s[0], q[0]);
+            s_stats[wg * N + c0 + 8] = make_float2(s[1], q[1]);
+        }
+        flush_tile_stats<N, 2>(P, s_stats, t.img, t.n_idx);
     }
 }
 
@@ -446,10 +512,25 @@ __device__ __forceinline__ void epilogue_fused(const ConvParams& P, float* acc, 
 // product + one e4m3 wgmma on the lo pair blocks (A entries then hold [A_hi | A_lo8], B entries [B_hi | B_lo8]).
 enum { MODE_FP16 = 0, MODE_FP16X3 = 1, MODE_F8 = 2 };
 
-template <int N_TILE, int MODE, bool FUSED>
+// One fp16 wgmma step of the tile: activation rows x weight rows, or (SWAP) weight rows x activation rows on 128 pixels.
+template <int N_TILE, bool SWAP>
+__device__ __forceinline__ void mma_f16(float* d, uint64_t act, uint64_t w) {
+    if constexpr (SWAP) wgmma_f16<128>(d, w, act);
+    else                wgmma_f16<N_TILE>(d, act, w);
+}
+template <int N_TILE, bool SWAP>
+__device__ __forceinline__ void mma_e4m3(float* d, uint64_t act, uint64_t w) {
+    if constexpr (SWAP) wgmma_e4m3<128>(d, w, act);
+    else                wgmma_e4m3<N_TILE>(d, act, w);
+}
+
+template <int N_TILE, int MODE, bool FUSED, bool SWAP>
 __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constant__ ConvParams P)
 {
+    static_assert(!SWAP || (N_TILE == SWAP_N_TILE && !FUSED), "the swapped orientation is the N = 64, unfused kernel");
     constexpr bool SPLIT = MODE != MODE_FP16;
+    constexpr int TH = SWAP ? SWAP_TILE_H : TILE_H;                  // tile rows; each consumer warpgroup owns half
+    constexpr int ACC = SWAP ? 64 : N_TILE / 2;                       // fp32 accumulators per consumer thread
     using C = Cfg<N_TILE, SPLIT>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -495,7 +576,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
         }
         int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
         for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-            const TileCoord t = decode_tile(P, tile, m_tiles);
+            const TileCoord t = decode_tile<TH>(P, tile, m_tiles);
             for (int g = 0; g < P.ngroups; g++) {
                 const int first = P.g_first[g], cnt = P.g_cnt[g];
                 const int xx = t.x0 + P.dx[first], yy = t.y0 + P.dy[first];
@@ -529,21 +610,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
             }
         }
     } else if (warp < NUM_CONSUMERS / 32) {
-        // ================================ consumers (2 warpgroups, 64 tile rows each) ==================
+        // ================================ consumers (2 warpgroups, half of the tile rows each) ========
         const uint32_t smem_base = smem_u32(smem);
         const uint32_t b_base = smem_u32(b_ring);
-        const uint32_t a_row0 = (uint32_t)(warp >> 2) * 8u * ROW_BYTES;      // tile rows 8 g .. 8 g + 7
+        const uint32_t a_row0 = (uint32_t)(warp >> 2) * (TH / 2) * ROW_BYTES;   // tile rows (TH/2) g .. (TH/2)(g + 1) - 1
         // The e4m3 products get their own accumulator: Hopper's fp8 wgmma adds into D with a reduced-precision
         // accumulation, which would truncate the fp16 main product's fp32 sum.  The two are added in the epilogue.
-        float acc[N_TILE / 2];
-        float acc8[MODE == MODE_F8 ? N_TILE / 2 : 1];
+        float acc[ACC];
+        float acc8[MODE == MODE_F8 ? ACC : 1];
         int as = 0, bs = 0; uint32_t aph = 0, bph = 0;
         for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-            const TileCoord t = decode_tile(P, tile, m_tiles);
+            const TileCoord t = decode_tile<TH>(P, tile, m_tiles);
 #pragma unroll
-            for (int i = 0; i < N_TILE / 2; i++) acc[i] = 0.f;
+            for (int i = 0; i < ACC; i++) acc[i] = 0.f;
 #pragma unroll
-            for (int i = 0; i < (MODE == MODE_F8 ? N_TILE / 2 : 1); i++) acc8[i] = 0.f;
+            for (int i = 0; i < (MODE == MODE_F8 ? ACC : 1); i++) acc8[i] = 0.f;
             // B entry of the last committed wgmma group, and the A entry whose last tap is in that group: both are
             // released once the group has retired
             int prev_b = -1, prev_a = -1;
@@ -554,18 +635,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
                     const uint32_t a_hi = smem_base + as * a_stage_bytes + a_row0;
                     for (int i = 0; i < cnt; i++) {
                         mbar_wait(b_full + bs, bph);
-                        const uint32_t ai = a_hi + i * ROW_BYTES, al = ai + a_op_bytes;      // tap i: rows i .. i + 15
+                        const uint32_t ai = a_hi + i * ROW_BYTES, al = ai + a_op_bytes;      // tap i: rows i .. i + TH/2 - 1
                         const uint32_t b_hi = b_base + bs * C::B_STAGE_BYTES, b_lo = b_hi + C::B_BYTES;
                         wgmma_fence();
 #pragma unroll
                         for (int k = 0; k < KCHUNK / 16; k++) {
                             const uint64_t da = make_desc(ai + k * 32), db = make_desc(b_hi + k * 32);
-                            wgmma_f16<N_TILE>(acc, da, db);
+                            mma_f16<N_TILE, SWAP>(acc, da, db);
                             if constexpr (MODE == MODE_F8) {
-                                wgmma_e4m3<N_TILE>(acc8, make_desc(al + k * 32), make_desc(b_lo + k * 32));
+                                mma_e4m3<N_TILE, SWAP>(acc8, make_desc(al + k * 32), make_desc(b_lo + k * 32));
                             } else if constexpr (MODE == MODE_FP16X3) {
-                                wgmma_f16<N_TILE>(acc, da, make_desc(b_lo + k * 32));
-                                wgmma_f16<N_TILE>(acc, make_desc(al + k * 32), db);
+                                mma_f16<N_TILE, SWAP>(acc, da, make_desc(b_lo + k * 32));
+                                mma_f16<N_TILE, SWAP>(acc, make_desc(al + k * 32), db);
                             }
                         }
                         wgmma_commit();
@@ -587,14 +668,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
             }
             wgmma_wait<0>();
 #pragma unroll
-            for (int i = 0; i < N_TILE / 2; i++) acc_fence(acc[i]);
+            for (int i = 0; i < ACC; i++) acc_fence(acc[i]);
             if constexpr (MODE == MODE_F8) {
 #pragma unroll
-                for (int i = 0; i < N_TILE / 2; i++) { acc_fence(acc8[i]); acc[i] += acc8[i]; }
+                for (int i = 0; i < ACC; i++) { acc_fence(acc8[i]); acc[i] += acc8[i]; }
             }
             if (lane == 0) { mbar_arrive(b_empty + prev_b); mbar_arrive(a_empty + prev_a); }
-            if constexpr (FUSED) epilogue_fused<N_TILE>(P, acc, t, warp, lane, s_stats, s_ss);
-            else                 epilogue_plain<N_TILE>(P, acc, t, warp, lane, s_stats);
+            if constexpr (SWAP)       epilogue_swapped(P, acc, t, warp, lane, s_stats);
+            else if constexpr (FUSED) epilogue_fused<N_TILE>(P, acc, t, warp, lane, s_stats, s_ss);
+            else                      epilogue_plain<N_TILE>(P, acc, t, warp, lane, s_stats);
         }
     }
 }
@@ -646,17 +728,20 @@ struct Launch {
     int grid;
 };
 
+// N tile 64 always runs the swapped orientation (256-pixel tiles, see the top of the file); plan creation sized its
+// tiles and boxes with tile_rows(n_tile) to match.
 template <int N_TILE, int MODE, bool FUSED>
 int launch_wg(const Launch& L, cudaStream_t st)
 {
     using C = Cfg<N_TILE, MODE != MODE_FP16>;
+    constexpr bool SWAP = N_TILE == SWAP_N_TILE;
     static bool attr_set_dev[lwb::kMaxDevices] = {};          // function attributes are per device
     bool& attr_set = attr_set_dev[lwb::device_slot()];
     if (!attr_set) {
-        LWB_CUDA_OK(cudaFuncSetAttribute(k_conv_wg<N_TILE, MODE, FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        LWB_CUDA_OK(cudaFuncSetAttribute(k_conv_wg<N_TILE, MODE, FUSED, SWAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
         attr_set = true;
     }
-    LWB_CUDA_OK(lwb::launch_pdl(k_conv_wg<N_TILE, MODE, FUSED>, dim3(L.grid), dim3(NUM_THREADS), C::SMEM_BYTES, st, L.p));
+    LWB_CUDA_OK(lwb::launch_pdl(k_conv_wg<N_TILE, MODE, FUSED, SWAP>, dim3(L.grid), dim3(NUM_THREADS), C::SMEM_BYTES, st, L.p));
     LWB_LAUNCH_OK();
     return LWB_OK;
 }
@@ -720,8 +805,9 @@ static int map_nhwc_parity(CUtensorMap* m, const uint16_t* base, int n, int h, i
 
 // Orders the taps of p into y-halo groups: taps that read the same input view (tmap) at the same dx with consecutive
 // ascending dy share one activation box (at most MAX_GROUP taps per group; a tap that matches nothing is a group of
-// one).  wtap keeps addressing the weights, so the order of the taps is free.  Sets the groups and a_rows.
-static void group_taps(ConvParams& p)
+// one).  wtap keeps addressing the weights, so the order of the taps is free.  Sets the groups and a_rows (boxes of
+// tile_h output rows plus the group's halo).
+static void group_taps(ConvParams& p, int tile_h)
 {
     int order[MAX_TAPS];
     for (int t = 0; t < p.ntaps; t++) order[t] = t;
@@ -742,16 +828,17 @@ static void group_taps(ConvParams& p)
         p.g_cnt[p.ngroups - 1]++;
         longest = std::max(longest, (int)p.g_cnt[p.ngroups - 1]);
     }
-    p.a_rows = TILE_H + longest - 1;
+    p.a_rows = tile_h + longest - 1;
 }
 
 // Ring depths inside RING_BYTES: at least two entries per ring (the consumers release an entry one wgmma group late),
-// otherwise the split that keeps the most taps in flight, min(A entries x longest group, B entries).
+// otherwise the split that keeps the most taps in flight, min(A entries x longest group, B entries).  With the 32-row
+// tiles of the swapped orientation the activation entry is the large one (fp16f8 3x3: 2 x 68 KB A + 4 x 16 KB B).
 static void pick_rings(ConvParams& p, int n_tile, bool split)
 {
     const int ops = split ? 2 : 1;
     const int a_bytes = p.a_rows * ROW_BYTES * ops, b_bytes = n_tile * 128 * ops;
-    const int longest = p.a_rows - TILE_H + 1;
+    const int longest = p.a_rows - tile_rows(n_tile) + 1;
     int best = 0;
     for (int a = 2; a <= MAX_STAGES; a++) {
         const int b = std::min(MAX_STAGES, (RING_BYTES - a * a_bytes) / b_bytes);
@@ -795,7 +882,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         ConvParams& p = L.p;
         p.n_img = d->n;
         p.dom_h = dom_h; p.dom_w = dom_w;
-        p.tiles_y = lwb::ceil_div(dom_h, TILE_H); p.tiles_x = lwb::ceil_div(dom_w, TILE_W);
+        p.tiles_y = lwb::ceil_div(dom_h, tile_rows(n_tile)); p.tiles_x = lwb::ceil_div(dom_w, TILE_W);
         p.n_tiles_n = d->cout / n_tile;
         p.out = out_raw; p.out_h = d->h_out; p.out_w = d->w_out; p.cout = d->cout;
         p.stats = stats;
@@ -816,7 +903,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         memset(&L.p, 0, sizeof(L.p));
         L.p.ntaps = d->kh; L.p.chunks0 = 1; L.p.chunks1 = 0;
         for (int ky = 0; ky < d->kh; ky++) { L.p.dy[ky] = (signed char)ky; L.p.dx[ky] = 0; L.p.tmap[ky] = 0; L.p.wtap[ky] = (short)ky; }
-        group_taps(L.p);
+        group_taps(L.p, tile_rows(n_tile));
         const int hp = d->h_in + d->kh - 1;
         const uint64_t dims[4] = {64, (uint64_t)d->w_in, (uint64_t)hp, (uint64_t)d->n};
         const uint64_t str[3] = {16, (uint64_t)d->row_pitch * 16, (uint64_t)hp * d->row_pitch * 16};
@@ -850,13 +937,13 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         LWB_CHECK_ARG(d->kh == 3 && d->kw == 3 && d->stride == 2 && d->pad == 1 && d->cin1 == 0, "transposed conv: only k3 s2 p1 op1");
         LWB_CHECK_ARG(d->h_out == 2 * d->h_in && d->w_out == 2 * d->w_in, "transposed conv output must be 2x input");
         const int ncols = 4 * d->cout;
-        n_tile = ncols % 128 == 0 ? 128 : 64;
+        n_tile = MAX_N_TILE;                                  // the swapped N = 64 epilogue has no phase columns
         LWB_CHECK_ARG(d->cout % 32 == 0 && ncols % n_tile == 0, "merged transposed conv needs cout in multiples of 32");
         Launch& L = plan->launches[plan->num++];
         memset(&L.p, 0, sizeof(L.p));
         for (int t = 0; t < 4; t++) { L.p.dy[t] = (signed char)(t >> 1); L.p.dx[t] = (signed char)(t & 1); L.p.tmap[t] = 0; L.p.wtap[t] = (short)t; }
         L.p.ntaps = 4; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = 0;
-        group_taps(L.p);
+        group_taps(L.p, tile_rows(n_tile));
         if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
         if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
         const uint64_t mwd[3] = {(uint64_t)cin_total, (uint64_t)ncols, 4};
@@ -890,7 +977,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
                 t++;
             }
             L.p.ntaps = t; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = 0;
-            group_taps(L.p);
+            group_taps(L.p, tile_rows(n_tile));
             if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
             if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
             if ((rc = encode_map(&L.p.w_hi, w_hi, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
@@ -923,7 +1010,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     }
     L.p.ntaps = t; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = d->cin1 / KCHUNK;
     L.p.oy_mul = 1; L.p.ox_mul = 1; L.p.oy_add = 0; L.p.ox_add = 0;
-    group_taps(L.p);
+    group_taps(L.p, tile_rows(n_tile));
     const int rows = L.p.a_rows;
     if (d->stride == 1) {
         if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, rows)) != LWB_OK) return fail(rc);

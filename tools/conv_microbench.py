@@ -3,8 +3,9 @@
 The layers are the ones the flagship step runs (256x256, 16 frames as two sub-batch streams of 8), each in the three
 operand modes: fp16f8 (the default, split=2), fp16x3 (split=1) and single-pass fp16 (split=0).  The row-K stem has no
 fp8 path and runs fp16x3 where fp16f8 is asked for, as in the generator.  Beside the time, every layer prints the
-operand bytes per algorithmic FLOP that the TMA unit moves from L2 into shared memory: once for a schedule that fetches
-a 16-row activation tile per filter tap ("per-tap") and once for the y-halo tap groups the engine runs ("grouped").
+operand bytes per algorithmic FLOP that the TMA unit moves from L2 into shared memory: for a schedule that fetches a
+16-row activation tile per filter tap ("tap"), for y-halo tap groups on 16 x 8 tiles ("grp16"), and for the tiles the
+engine runs ("run"): the same 16 x 8 tiles for N tiles of 16..128, the swapped 32 x 8 tiles for an N tile of 64.
 
     python tools/conv_microbench.py [--batch 8] [--reps 50] [--only res] [--json out.json]
 """
@@ -19,6 +20,11 @@ from impersonator_b200 import kernels as K  # noqa: E402
 from impersonator_b200.generator import merge_transposed_weight  # noqa: E402
 
 TILE_H, TILE_W, KCHUNK, MAX_GROUP = 16, 8, 64, 8
+SWAP_N_TILE, SWAP_TILE_H = 64, 32            # N = 64 plans run 64 channels x (32 x 8) pixels
+
+
+def tile_rows(n_tile):
+    return SWAP_TILE_H if n_tile == SWAP_N_TILE else TILE_H
 MODES = (("fp16f8", 2), ("fp16x3", 1), ("fp16", 0))
 
 
@@ -61,20 +67,20 @@ def launch_taps(spec):
     return [taps]
 
 
-def operand_bytes(spec, n, n_tile, split, grouped):
-    """TMA bytes of the whole layer (A hi/lo + B hi/lo, every tile)."""
+def operand_bytes(spec, n, n_tile, split, grouped, tile_h=TILE_H):
+    """TMA bytes of the whole layer (activation hi/lo + weight hi/lo, every tile of tile_h x 8 pixels)."""
     ops = 2 if split else 1
     chunks = 1 if spec["kind"] == "rowk" else (spec["cin"] + spec.get("cin1", 0)) // KCHUNK
     dom = spec["h"] // 2 if spec.get("stride", 1) == 2 else spec["h"]
     ncols = 4 * spec["cout"] if spec["kind"] == "merged" else spec["cout"]
-    tiles = n * -(-dom // TILE_H) * -(-dom // TILE_W) * (ncols // n_tile)
+    tiles = n * -(-dom // tile_h) * -(-dom // TILE_W) * (ncols // n_tile)
     total = 0
     for taps in launch_taps(spec):
         if grouped:
             groups, longest = tap_groups(taps)
-            a_rows = groups * (TILE_H + longest - 1)
+            a_rows = groups * (tile_h + longest - 1)
         else:
-            a_rows = len(taps) * TILE_H
+            a_rows = len(taps) * tile_h
         total += tiles * chunks * ops * (a_rows * TILE_W * 128 + len(taps) * n_tile * 128)
     return total
 
@@ -166,7 +172,8 @@ def main():
     torch.manual_seed(0)
     torch.set_grad_enabled(False)
     rows = []
-    print("%-34s %-7s %9s %9s %10s %10s" % ("layer (batch %d)" % a.batch, "mode", "ms", "TFLOP/s", "B/FLOP tap", "B/FLOP grp"))
+    print("%-34s %-7s %9s %9s %10s %10s %10s" % ("layer (batch %d)" % a.batch, "mode", "ms", "TFLOP/s", "B/FLOP tap",
+                                                  "B/FLOP g16", "B/FLOP run"))
     for name, spec in LAYERS:
         if a.only and a.only not in name:
             continue
@@ -175,10 +182,13 @@ def main():
             ms = time_plan(plan, a.reps)
             n_tile = spec.get("n_tile") or (128 if (4 * spec["cout"] if spec["kind"] == "merged" else spec["cout"]) % 128 == 0 else 64)
             bpf = [operand_bytes(spec, a.batch, n_tile, ran, g) / plan.flops for g in (False, True)]
-            row = dict(layer=name, mode=mode, ran_split=ran, ms=ms, tflops=plan.flops / ms / 1e9,
-                       bytes_per_flop_per_tap=bpf[0], bytes_per_flop_grouped=bpf[1])
+            bpf.append(operand_bytes(spec, a.batch, n_tile, ran, True, tile_rows(n_tile)) / plan.flops)
+            row = dict(layer=name, mode=mode, ran_split=ran, ms=ms, tflops=plan.flops / ms / 1e9, n_tile=n_tile,
+                       tile_h=tile_rows(n_tile), bytes_per_flop_per_tap=bpf[0], bytes_per_flop_grouped=bpf[1],
+                       bytes_per_flop_run=bpf[2])
             rows.append(row)
-            print("%-34s %-7s %9.4f %9.1f %10.4f %10.4f" % (name, mode + ("*" if ran != split else ""), ms, row["tflops"], bpf[0], bpf[1]))
+            print("%-34s %-7s %9.4f %9.1f %10.4f %10.4f %10.4f" % (name, mode + ("*" if ran != split else ""), ms, row["tflops"],
+                                                                  bpf[0], bpf[1], bpf[2]))
             del plan
     print("* the row-K stem has no fp8 path: fp16x3 operands")
     props = torch.cuda.get_device_properties(0)
