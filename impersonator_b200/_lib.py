@@ -27,16 +27,6 @@ class ConvDesc(ctypes.Structure):
         "kh", "kw", "stride", "pad", "dil", "transposed", "split", "rowk", "row_pitch", "n_tile", "halo", "w_exp", "pad_w")]
 
 
-class FusedNorm(ctypes.Structure):
-    """struct lwb_fused_norm (include/lwb_b200.h)."""
-    _fields_ = [("gamma", ctypes.c_void_p), ("beta", ctypes.c_void_p), ("eps", ctypes.c_float), ("relu", ctypes.c_int),
-                ("residual", ctypes.c_void_p),
-                ("warp_src", ctypes.c_void_p), ("src_batch", ctypes.c_int), ("T", ctypes.c_void_p), ("th", ctypes.c_int),
-                ("tw", ctypes.c_int), ("align_corners", ctypes.c_int),
-                ("y_f32", ctypes.c_void_p), ("y_hi", ctypes.c_void_p), ("y_lo", ctypes.c_void_p), ("lo_format", ctypes.c_int),
-                ("range_flag", ctypes.c_void_p), ("counters", ctypes.c_void_p)]
-
-
 _vp, _i, _f, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_size_t
 
 # name -> (restype, argtypes); must list EVERY symbol include/lwb_b200.h declares (tests check it).
@@ -56,7 +46,6 @@ SIGNATURES = {
     "lwb_nhwc_to_nchw": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "lwb_conv_plan_create": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                   ctypes.POINTER(_vp)]),
-    "lwb_conv_plan_fuse_norm": (_i, [_vp, ctypes.POINTER(FusedNorm)]),
     "lwb_conv_plan_run": (_i, [_vp, _vp]),
     "lwb_conv_plan_num_launches": (_i, [_vp]),
     "lwb_conv_plan_destroy": (None, [_vp]),

@@ -43,8 +43,7 @@
 //                   NHWC8 row are 64 contiguous fp16, so one K = 64 stage covers a whole filter
 //                   row (overlapping-stride tensor map); 7 stages instead of 49.
 // Epilogue: accumulator registers -> fp32 NHWC global + per-(n, c) sum / sum of squares for the
-// InstanceNorm that follows every conv (lane shuffles -> smem -> one f64 atomic per column per tile),
-// or (FUSED) the InstanceNorm itself, see epilogue_fused.
+// InstanceNorm that follows every conv (lane shuffles -> smem -> one f64 atomic per column per tile).
 #include <cuda.h>
 
 #include <stdlib.h>
@@ -52,10 +51,7 @@
 #include <algorithm>
 #include <new>
 
-#include <cuda_fp8.h>
-
 #include "common.cuh"
-#include "sample.cuh"
 
 namespace {
 
@@ -79,21 +75,7 @@ static_assert(SWAP_N_TILE * (SWAP_TILE_H * TILE_W) == MAX_N_TILE * (TILE_H * TIL
 
 __host__ __device__ constexpr int tile_rows(int n_tile) { return n_tile == SWAP_N_TILE ? SWAP_TILE_H : TILE_H; }
 
-// InstanceNorm (+ReLU, +residual, +LWB warp-add) fused into the conv epilogue (k_conv_wg<.., FUSED = true>): the operands
-// of the NEXT layer leave the kernel directly, no fp32 raw tensor and no second pass over HBM.  See epilogue_fused.
-struct FusedNorm {
-    const float* gamma; const float* beta; float eps; int relu;
-    const float* residual;                                // [n,h,w,c] fp32, nullable
-    const float* warp_src; int src_batch; const float* T; int th, tw, align_corners;      // nullable LWB source (NHWC fp32)
-    float* y_f32; __half* y_hi; uint8_t* y_lo; int lo_format;
-    int* range_flag;
-    int* counters;                                        // [n_img * n_tiles_n], zero before every run: tiles of a unit done
-    int tiles_per_image;
-    double inv_hw;
-};
-
 struct ConvParams {
-    FusedNorm fn;
     CUtensorMap a_hi[4];
     CUtensorMap a_lo[4];
     CUtensorMap w_hi;
@@ -116,15 +98,14 @@ struct ConvParams {
 };
 
 // Shared memory: [A ring: a_stages x (hi | lo) boxes of a_rows rows][B ring: b_stages x (hi | lo) weight tiles] inside
-// RING_BYTES, then the barriers, the statistics partials and (fused mode) the per-channel scale / shift.
+// RING_BYTES, then the barriers and the statistics partials.
 template <int N_TILE, bool SPLIT>
 struct Cfg {
     static constexpr int B_BYTES = N_TILE * 128;
     static constexpr int B_STAGE_BYTES = B_BYTES * (SPLIT ? 2 : 1);
     static constexpr int BAR_BYTES = 4 * MAX_STAGES * 8;         // A full / empty, B full / empty
     static constexpr int STATS_BYTES = 8 * N_TILE * 8;           // [8 consumer warps][N_TILE] float2
-    static constexpr int SS_BYTES = N_TILE * 8;                  // [N_TILE] (scale, shift), fused mode
-    static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + STATS_BYTES + SS_BYTES;
+    static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + STATS_BYTES;
     static_assert(B_STAGE_BYTES % 1024 == 0, "B entries must keep the 1024-byte swizzle alignment");
     static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the shared memory of a block");
 };
@@ -389,124 +370,6 @@ __device__ __forceinline__ void epilogue_swapped(const ConvParams& P, float* acc
     }
 }
 
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
-    int v;
-    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ uint8_t cvt_e4m3(float v) { return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3); }
-
-// Fused epilogue.  A "unit" = (image, N tile): its InstanceNorm statistics need every M tile of the image.  Each CTA
-// (a) reduces its tile's per-channel sum / sum of squares and adds them to the global f64 statistics, (b) publishes
-// "tile done" on the unit's counter and waits until all tiles_per_image tiles are in, (c) reads the finished statistics,
-// and (d) normalises its tile, applying ReLU / residual / LWB warp-add and writing the next layer's operands (fp16 hi +
-// fp16 or e4m3-pair lo, optional fp32).
-// Why the wait cannot deadlock: the grid is persistent with one CTA per SM (all CTAs co-resident), tiles are taken in
-// rounds of gridDim.x and a unit is a run of consecutive tiles no longer than one round, so a CTA holds at most one tile
-// of a unit.  Every tile of the lowest unfinished unit belongs to a CTA whose earlier tiles all lie in finished units: it
-// reaches that tile and publishes it.  The host enables this mode only when tiles_per_image <= gridDim.x and never
-// together with multi-stream sub-batches.
-template <int N_TILE>
-__device__ __forceinline__ void epilogue_fused(const ConvParams& P, float* acc, const TileCoord& t, int warp, unsigned lane,
-                                               float2* s_stats, float2* s_ss)
-{
-    const FusedNorm& F = P.fn;
-    const int tx = (int)(lane >> 2), x = t.x0 + tx;
-    const int y[2] = {t.y0 + 2 * warp, t.y0 + 2 * warp + 1};
-    const bool valid[2] = {y[0] < P.dom_h && x < P.dom_w, y[1] < P.dom_h && x < P.dom_w};
-#pragma unroll
-    for (int i = 0; i < N_TILE / 2; i++) acc[i] *= P.out_scale;
-    // ---- pass 1: per-channel sums of this tile -> global statistics
-    warp_tile_stats<N_TILE>(acc, valid[0], valid[1], warp, lane, s_stats);
-    flush_tile_stats<N_TILE>(P, s_stats, t.img, t.n_idx);
-    __threadfence();
-    consumer_sync();
-    // ---- publish + wait for the unit
-    if (threadIdx.x == 0) {
-        int* ctr = F.counters + t.img * P.n_tiles_n + t.n_idx;
-        atomicAdd(ctr, 1);
-        if (ld_acquire_gpu(ctr) < F.tiles_per_image) {
-            const long long t0 = clock64();
-            while (ld_acquire_gpu(ctr) < F.tiles_per_image) {
-                __nanosleep(64);
-                if (clock64() - t0 > 4000000000ll) __trap();          // no printf: see mbar_wait
-            }
-        }
-    }
-    consumer_sync();
-    for (int col = threadIdx.x; col < N_TILE; col += NUM_CONSUMERS) {
-        const int ch = t.n_idx * N_TILE + col;
-        const double* sp = P.stats + 2 * ((size_t)t.img * P.cout + ch);
-        const double mean = __ldcg(sp) * F.inv_hw;
-        double var = __ldcg(sp + 1) * F.inv_hw - mean * mean;
-        if (var < 0) var = 0;
-        const float rstd = (float)(1.0 / sqrt(var + (double)F.eps));
-        const float g = F.gamma ? __ldg(F.gamma + ch) : 1.f, bt = F.beta ? __ldg(F.beta + ch) : 0.f;
-        s_ss[col] = make_float2(g * rstd, bt - (float)mean * g * rstd);
-    }
-    consumer_sync();
-    // ---- pass 2: normalise this thread's two pixels, emit operands
-    unsigned hmax = 0;
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-        if (!valid[h]) continue;
-        const size_t pix = ((size_t)t.img * P.out_h + y[h]) * P.out_w + x;      // fused plans have oy_mul = ox_mul = 1
-        lwb::Taps tp;
-        tp.m = 0;
-        if (F.warp_src) {
-            float gx, gy;
-            lwb::flow_at(F.T + (size_t)t.img * F.th * F.tw * 2, F.th, F.tw, P.out_h, P.out_w, y[h], x, gx, gy);
-            lwb::make_taps(gx, gy, P.out_h, P.out_w, F.align_corners, tp);
-        }
-        const float* wsrc = F.warp_src ? F.warp_src + (size_t)(F.src_batch == 1 ? 0 : t.img) * P.out_h * P.out_w * P.cout : nullptr;
-        const int offs[4] = {tp.o00, tp.o00 + 1, tp.o00 + P.out_w, tp.o00 + P.out_w + 1};
-        const float wt[4] = {tp.w00, tp.w01, tp.w10, tp.w11};
-#pragma unroll
-        for (int j = 0; j < N_TILE / 8; j++) {
-            const int c = 8 * j + 2 * (int)(lane & 3);
-            const int ch0 = t.n_idx * N_TILE + c;
-            const float2 ss0 = s_ss[c], ss1 = s_ss[c + 1];
-            float v0 = fmaf(acc[4 * j + 2 * h], ss0.x, ss0.y), v1 = fmaf(acc[4 * j + 2 * h + 1], ss1.x, ss1.y);
-            if (F.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            if (F.residual) {
-                const float2 r = __ldg(reinterpret_cast<const float2*>(F.residual + pix * P.cout + ch0));
-                v0 += r.x; v1 += r.y;
-            }
-            if (tp.m) {
-                float w0 = 0.f, w1 = 0.f;
-#pragma unroll
-                for (int t4 = 0; t4 < 4; t4++) {
-                    if (tp.m & (1 << t4)) {
-                        const float2 s = __ldg(reinterpret_cast<const float2*>(wsrc + (size_t)offs[t4] * P.cout + ch0));
-                        w0 += s.x * wt[t4]; w1 += s.y * wt[t4];
-                    }
-                }
-                v0 += w0; v1 += w1;
-            }
-            if (F.y_f32) *reinterpret_cast<float2*>(F.y_f32 + pix * P.cout + ch0) = make_float2(v0, v1);
-            if (F.y_hi) {
-                const __half2 hh = __halves2half2(__float2half_rn(v0), __float2half_rn(v1));
-                *reinterpret_cast<__half2*>(F.y_hi + pix * P.cout + ch0) = hh;
-                hmax = __vmaxu2(hmax, *reinterpret_cast<const unsigned*>(&hh) & 0x7fff7fffu);
-                const float l0 = v0 - __low2float(hh), l1 = v1 - __high2float(hh);
-                if (F.y_lo && F.lo_format == 0) {
-                    *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(F.y_lo) + pix * P.cout + ch0) =
-                        __halves2half2(__float2half_rn(l0), __float2half_rn(l1));
-                } else if (F.y_lo) {
-                    // e4m3 pair block of this pixel's 64-channel group: bytes [ch % 64] = e4m3(x / 16), [64 + ch % 64] = e4m3(x_lo * 2^10)
-                    uint8_t* blk = F.y_lo + (pix * P.cout + (size_t)(ch0 & ~63)) * 2 + (ch0 & 63);
-                    *reinterpret_cast<uint16_t*>(blk) = (uint16_t)(cvt_e4m3(v0 * (1.f / 16.f)) | (cvt_e4m3(v1 * (1.f / 16.f)) << 8));
-                    *reinterpret_cast<uint16_t*>(blk + 64) = (uint16_t)(cvt_e4m3(l0 * 1024.f) | (cvt_e4m3(l1 * 1024.f) << 8));
-                }
-            }
-        }
-    }
-    if (F.range_flag) {
-        const unsigned m = max(hmax & 0xffffu, hmax >> 16);
-        if (m >= 0x6400u) atomicOr(F.range_flag, m >= 0x7b53u ? 3 : 1);
-    }
-}
-
 // ----------------------------------------------------------------------------------- kernel
 // Operand modes (lwb_conv_desc.split): one fp16 product, the three fp16 products of the hi/lo split, or the fp16 hi
 // product + one e4m3 wgmma on the lo pair blocks (A entries then hold [A_hi | A_lo8], B entries [B_hi | B_lo8]).
@@ -524,10 +387,12 @@ __device__ __forceinline__ void mma_e4m3(float* d, uint64_t act, uint64_t w) {
     else                wgmma_e4m3<N_TILE>(d, act, w);
 }
 
-template <int N_TILE, int MODE, bool FUSED, bool SWAP>
+template <int N_TILE, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constant__ ConvParams P)
 {
-    static_assert(!SWAP || (N_TILE == SWAP_N_TILE && !FUSED), "the swapped orientation is the N = 64, unfused kernel");
+    // N tile 64 always runs the swapped orientation (256-pixel tiles, see the top of the file); plan creation sized its
+    // tiles and boxes with tile_rows(n_tile) to match.
+    constexpr bool SWAP = N_TILE == SWAP_N_TILE;
     constexpr bool SPLIT = MODE != MODE_FP16;
     constexpr int TH = SWAP ? SWAP_TILE_H : TILE_H;                  // tile rows; each consumer warpgroup owns half
     constexpr int ACC = SWAP ? 64 : N_TILE / 2;                       // fp32 accumulators per consumer thread
@@ -542,7 +407,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
     uint64_t* b_full = a_empty + MAX_STAGES;
     uint64_t* b_empty = b_full + MAX_STAGES;
     float2* s_stats = reinterpret_cast<float2*>(smem + RING_BYTES + C::BAR_BYTES);   // [8][N_TILE]
-    float2* s_ss = s_stats + 8 * N_TILE;                                             // [N_TILE]
 
     const int warp = threadIdx.x >> 5;
     const unsigned lane = threadIdx.x & 31;
@@ -674,9 +538,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
                 for (int i = 0; i < ACC; i++) { acc_fence(acc8[i]); acc[i] += acc8[i]; }
             }
             if (lane == 0) { mbar_arrive(b_empty + prev_b); mbar_arrive(a_empty + prev_a); }
-            if constexpr (SWAP)       epilogue_swapped(P, acc, t, warp, lane, s_stats);
-            else if constexpr (FUSED) epilogue_fused<N_TILE>(P, acc, t, warp, lane, s_stats, s_ss);
-            else                      epilogue_plain<N_TILE>(P, acc, t, warp, lane, s_stats);
+            if constexpr (SWAP) epilogue_swapped(P, acc, t, warp, lane, s_stats);
+            else                epilogue_plain<N_TILE>(P, acc, t, warp, lane, s_stats);
         }
     }
 }
@@ -724,24 +587,20 @@ struct Launch {
     ConvParams p;
     int n_tile;
     int mode;
-    bool fused;
     int grid;
 };
 
-// N tile 64 always runs the swapped orientation (256-pixel tiles, see the top of the file); plan creation sized its
-// tiles and boxes with tile_rows(n_tile) to match.
-template <int N_TILE, int MODE, bool FUSED>
+template <int N_TILE, int MODE>
 int launch_wg(const Launch& L, cudaStream_t st)
 {
     using C = Cfg<N_TILE, MODE != MODE_FP16>;
-    constexpr bool SWAP = N_TILE == SWAP_N_TILE;
     static bool attr_set_dev[lwb::kMaxDevices] = {};          // function attributes are per device
     bool& attr_set = attr_set_dev[lwb::device_slot()];
     if (!attr_set) {
-        LWB_CUDA_OK(cudaFuncSetAttribute(k_conv_wg<N_TILE, MODE, FUSED, SWAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        LWB_CUDA_OK(cudaFuncSetAttribute(k_conv_wg<N_TILE, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
         attr_set = true;
     }
-    LWB_CUDA_OK(lwb::launch_pdl(k_conv_wg<N_TILE, MODE, FUSED, SWAP>, dim3(L.grid), dim3(NUM_THREADS), C::SMEM_BYTES, st, L.p));
+    LWB_CUDA_OK(lwb::launch_pdl(k_conv_wg<N_TILE, MODE>, dim3(L.grid), dim3(NUM_THREADS), C::SMEM_BYTES, st, L.p));
     LWB_LAUNCH_OK();
     return LWB_OK;
 }
@@ -749,12 +608,9 @@ int launch_wg(const Launch& L, cudaStream_t st)
 template <int N_TILE>
 int launch_one(const Launch& L, cudaStream_t st)
 {
-    if constexpr (N_TILE == MAX_N_TILE) {
-        if (L.fused) return L.mode == MODE_F8 ? launch_wg<N_TILE, MODE_F8, true>(L, st) : launch_wg<N_TILE, MODE_FP16X3, true>(L, st);
-    }
-    if (L.mode == MODE_F8) return launch_wg<N_TILE, MODE_F8, false>(L, st);
-    if (L.mode == MODE_FP16X3) return launch_wg<N_TILE, MODE_FP16X3, false>(L, st);
-    return launch_wg<N_TILE, MODE_FP16, false>(L, st);
+    if (L.mode == MODE_F8) return launch_wg<N_TILE, MODE_F8>(L, st);
+    if (L.mode == MODE_FP16X3) return launch_wg<N_TILE, MODE_FP16X3>(L, st);
+    return launch_wg<N_TILE, MODE_FP16>(L, st);
 }
 
 int launch(const Launch& L, cudaStream_t st)
@@ -887,7 +743,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         p.out = out_raw; p.out_h = d->h_out; p.out_w = d->w_out; p.cout = d->cout;
         p.stats = stats;
         p.out_scale = f8 ? ldexpf(1.f, -d->w_exp) : 1.f;      // weights are packed x 2^w_exp in f8 mode (lwb_pack_conv_weight_f8)
-        L.n_tile = n_tile; L.mode = d->split; L.fused = false;
+        L.n_tile = n_tile; L.mode = d->split;
         pick_rings(p, n_tile, split);
         const long total = (long)p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
         L.grid = (int)(total < sms ? total : sms);
@@ -1029,37 +885,6 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
     finish(L, d->h_out, d->w_out);
     *plan_out = plan;
-    return LWB_OK;
-}
-
-extern "C" int lwb_conv_plan_fuse_norm(lwb_conv_plan* plan, const lwb_fused_norm* f)
-{
-    LWB_CHECK_ARG(plan && f, "null pointer");
-    if (plan->num != 1) { lwb::set_error("fuse_norm: multi-launch plans (transposed convs) keep the separate norm pass"); return LWB_E_UNSUPPORTED; }
-    Launch& L = plan->launches[0];
-    ConvParams& p = L.p;
-    if (L.mode == MODE_FP16 || L.n_tile != MAX_N_TILE || !p.stats || p.oy_mul != 1 || p.ox_mul != 1) {
-        lwb::set_error("fuse_norm: needs a split-mode plan with N tile %d and statistics", MAX_N_TILE);
-        return LWB_E_UNSUPPORTED;
-    }
-    const int tiles_per_image = p.tiles_y * p.tiles_x;
-    // every unit (image, N tile) must fit one round of the persistent grid (see epilogue_fused)
-    if (tiles_per_image > L.grid) {
-        lwb::set_error("fuse_norm: %d tiles per image exceed one round of the grid (%d CTAs)", tiles_per_image, L.grid);
-        return LWB_E_UNSUPPORTED;
-    }
-    LWB_CHECK_ARG(f->counters && (f->y_hi || f->y_f32), "fuse_norm: counters and an output are required");
-    LWB_CHECK_ARG(!f->warp_src || (f->T && f->th > 0 && f->tw > 0 && (f->src_batch == 1 || f->src_batch == p.n_img)), "bad warp arguments");
-    LWB_CHECK_ARG(f->lo_format == 0 || (f->lo_format == 1 && p.cout % 64 == 0), "lo_format 1 needs channels in blocks of 64");
-    FusedNorm& F = p.fn;
-    F.gamma = f->gamma; F.beta = f->beta; F.eps = f->eps; F.relu = f->relu;
-    F.residual = f->residual;
-    F.warp_src = f->warp_src; F.src_batch = f->src_batch; F.T = f->T; F.th = f->th; F.tw = f->tw; F.align_corners = f->align_corners;
-    F.y_f32 = f->y_f32; F.y_hi = (__half*)f->y_hi; F.y_lo = (uint8_t*)f->y_lo; F.lo_format = f->lo_format;
-    F.range_flag = f->range_flag;
-    F.counters = f->counters; F.tiles_per_image = tiles_per_image;
-    F.inv_hw = 1.0 / ((double)p.dom_h * p.dom_w);
-    L.fused = true;
     return LWB_OK;
 }
 

@@ -70,18 +70,6 @@ def _sub_batches(B, enc_w, res_w, bg):
     return n if shared else 1
 
 
-def _fuse_norm():
-    """LWB_FUSE_NORM (default 0 until measured faster): InstanceNorm (+ReLU / residual / LWB warp-add) of every eligible
-    layer (outputs up to 128 x 128, not transposed) runs inside the conv kernel's epilogue (lwb_conv_plan_fuse_norm) instead
-    of a separate pass.  The fused kernels' CTAs wait on each other, so the mode is mutually exclusive with LWB_STREAMS > 1."""
-    if os.environ.get("LWB_FUSE_NORM", "0") != "1":
-        return False
-    try:
-        return int(os.environ.get("LWB_STREAMS", "2")) <= 1
-    except ValueError:
-        return True
-
-
 def _tc_heads():
     """LWB_TC_HEADS (default 1): the 7x7 output heads run on the tensor cores as a 7x1 filter whose N dimension
     carries the 7 filter columns x 4 head channels (28 -> 32); the composite kernel sums the columns.  0 = the fp32
@@ -267,7 +255,7 @@ class _Act(object):
 
 class _Layer(object):
     """conv (+ InstanceNorm params) bound to buffers: plan + stats slot."""
-    __slots__ = ("plan", "raw", "stats", "gamma", "beta", "w", "wsrc", "counters", "fusable")
+    __slots__ = ("plan", "raw", "stats", "gamma", "beta", "w", "wsrc")
 
 
 class _StreamBase(object):
@@ -321,12 +309,9 @@ class _StreamBase(object):
         cmax = max(max(self._stats_slots), 16)
         # InstanceNorm statistics of every layer + the operand-range flag share one buffer: one fill per pass
         nstat = len(self._stats_slots) * self.B * cmax * 2
-        nctr = len(self._stats_slots) * self.B * 4                 # "tile done" counters of the fused-norm plans (<= 4 N tiles)
-        self._zero = torch.zeros(nstat * 8 + 8 + nctr * 4, dtype=torch.uint8, device=self.dev)
+        self._zero = torch.zeros(nstat * 8 + 4, dtype=torch.uint8, device=self.dev)
         self.stats = self._zero[:nstat * 8].view(torch.float64).view(len(self._stats_slots), self.B, cmax, 2)
-        self.range_flag = self._zero[nstat * 8:nstat * 8 + 4].view(torch.int32)
-        counters = self._zero[nstat * 8 + 8:].view(torch.int32).view(len(self._stats_slots), self.B * 4)
-        fuse = _fuse_norm()
+        self.range_flag = self._zero[nstat * 8:].view(torch.int32)
         self.ws = torch.empty((self.B, cmax, 2), dtype=torch.float32, device=self.dev)
         pend = [L for L in self._layers if L.wsrc is not None]
         if pend:
@@ -343,10 +328,6 @@ class _StreamBase(object):
                 self.stats[slot].view(-1)[:self.B * cout * 2].view(self.B, cout, 2)
             d, x0, x1 = L.plan
             L.plan = K.ConvPlan(d, x0, x1, L.w, L.raw, L.stats)
-            L.counters = counters[slot]
-            # eligibility is a property of the plan (probe with placeholder outputs; the real pointers are set per call)
-            L.fusable = bool(fuse and L.stats is not None and self.split != 0 and
-                             L.plan.fuse_norm(L.gamma, L.beta, True, L.counters, y_f32=L.raw))
 
     def _label_heads(self):
         """The folded heads issue N = 32 columns; their algorithmic work is the 7x7 x 64 -> 4 convolution."""
@@ -362,12 +343,6 @@ class _StreamBase(object):
         self.pass_id = _PASS[0]
 
     def _conv_norm(self, L, out, relu, residual=None, warp_src=None, T=None, ac=False):
-        if L.fusable:
-            L.plan.fuse_norm(L.gamma, L.beta, relu, L.counters, residual=residual, warp_src=warp_src, T=T, align_corners=ac,
-                             y_f32=out.f32, y_hi=out.hi, y_lo=out.lo, lo_format=1 if self.split == 2 else 0,
-                             range_flag=self.range_flag)
-            L.plan.run()
-            return
         L.plan.run()
         K.norm_act_nhwc(L.raw, L.stats, L.gamma, L.beta, relu, self.ws, residual=residual, warp_src=warp_src, T=T,
                         align_corners=ac, y_f32=out.f32, y_hi=out.hi, y_lo=out.lo, lo_format=1 if self.split == 2 else 0,

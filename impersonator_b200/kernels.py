@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ConvDesc, FusedNorm, LwbError, check, lib, ptr, stream, _chk_cuda
+from ._lib import ConvDesc, LwbError, check, lib, ptr, stream, _chk_cuda
 
 # utils/nmr.py:177: eye = [0, 0, -(1/tan(30 deg) + 1)], cast to float32 by look_at.py:33
 EYE_Z = float(np.float32(-(1. / np.tan(np.radians(30)) + 1)))
@@ -286,25 +286,6 @@ class ConvPlan(object):
             self.flops = 2.0 * d.n * d.h_out * d.w_out * d.cout * w[0].shape[0] * 7 * getattr(self, "_real_cin", 6)
         else:
             self.flops = 2.0 * d.n * d.h_out * d.w_out * d.cout * (d.cin0 + d.cin1) * d.kh * d.kw
-
-    def fuse_norm(self, gamma, beta, relu, counters, eps=1e-5, residual=None, warp_src=None, T=None, align_corners=False,
-                  y_f32=None, y_hi=None, y_lo=None, lo_format=0, range_flag=None):
-        """Fuse the following InstanceNorm (+ReLU/+residual/+LWB warp-add) into this plan's epilogue
-        (lwb_conv_plan_fuse_norm).  May be called again with new pointers before every run.  -> False when the plan is not
-        eligible (the caller keeps the separate norm_act_nhwc pass)."""
-        _chk_cuda(gamma, beta, residual, warp_src, T, y_f32, y_hi, y_lo, range_flag, counters)
-        f = FusedNorm(gamma=ptr(gamma), beta=ptr(beta), eps=eps, relu=1 if relu else 0, residual=ptr(residual),
-                      warp_src=ptr(warp_src), src_batch=warp_src.shape[0] if warp_src is not None else 0, T=ptr(T),
-                      th=T.shape[1] if T is not None else 0, tw=T.shape[2] if T is not None else 0,
-                      align_corners=1 if align_corners else 0, y_f32=ptr(y_f32), y_hi=ptr(y_hi), y_lo=ptr(y_lo),
-                      lo_format=int(lo_format), range_flag=ptr(range_flag), counters=ptr(counters))
-        rc = lib().lwb_conv_plan_fuse_norm(self._h, ctypes.byref(f))
-        if rc == -3:                                  # LWB_E_UNSUPPORTED
-            return False
-        check(rc, "lwb_conv_plan_fuse_norm")
-        self._fused_keep = (gamma, beta, residual, warp_src, T, y_f32, y_hi, y_lo, range_flag, counters)
-        self.fused = True
-        return True
 
     prof_class = "conv"                  # instrumentation class (bench.py breakdown); the folded heads report as "heads"
 

@@ -149,30 +149,13 @@ typedef struct lwb_conv_desc {
 /* A plan owns the TMA descriptors of one conv layer bound to fixed device buffers; creating it
  * costs a few driver calls, running it is one launch (four for a transposed conv).
  * out_raw = conv(x) (no bias); stats [n, cout, 2] f64 += per-(n,c) (sum, sum of squares) over
- * H*W (nullable; caller zero-fills) -- the InstanceNorm statistics, fused into the epilogue. */
+ * H*W (nullable; caller zero-fills) -- the InstanceNorm statistics, accumulated by the conv epilogue. */
 typedef struct lwb_conv_plan lwb_conv_plan;
 int  lwb_conv_plan_create(const lwb_conv_desc* d,
                           const uint16_t* x0_hi, const uint16_t* x0_lo,
                           const uint16_t* x1_hi, const uint16_t* x1_lo,
                           const uint16_t* w_hi, const uint16_t* w_lo,
                           float* out_raw, double* stats, lwb_conv_plan** plan);
-/* Fuse the InstanceNorm that follows the conv (+ReLU, +residual, +LWB warp-add: exactly lwb_norm_act_nhwc's arithmetic) into
- * the plan's epilogue: the kernel then writes the next layer's operands itself and out_raw stays untouched.  Needs a
- * split-mode plan with an N tile of 128 and stats whose every image fits one round of the persistent grid (at most one
- * tile of 16x8 pixels per CTA of the grid, i.e. per SM: 132 on an H100, e.g. <= 128x128 outputs) -- otherwise
- * LWB_E_UNSUPPORTED and the caller keeps the separate lwb_norm_act_nhwc pass.
- * counters: device int [n * cout / 128], zero before every lwb_conv_plan_run (like stats).
- * The kernel's CTAs wait on each other: do not run a fused plan concurrently with other kernels of comparable size on
- * other streams. */
-typedef struct lwb_fused_norm {
-    const float* gamma; const float* beta; float eps; int relu;
-    const float* residual;
-    const float* warp_src; int src_batch; const float* T; int th, tw, align_corners;
-    float* y_f32; uint16_t* y_hi; uint16_t* y_lo; int lo_format;
-    int* range_flag;
-    int* counters;
-} lwb_fused_norm;
-int  lwb_conv_plan_fuse_norm(lwb_conv_plan* plan, const lwb_fused_norm* f);
 int  lwb_conv_plan_run(const lwb_conv_plan* plan, lwb_stream_t stream);
 int  lwb_conv_plan_num_launches(const lwb_conv_plan* plan);
 void lwb_conv_plan_destroy(lwb_conv_plan* plan);

@@ -66,9 +66,6 @@ class ConvPlan(object):
         self.label = "emulated"
         self.prof_class = "conv"
 
-    def fuse_norm(self, *a, **k):
-        return False
-
     def run(self):
         d = self.desc
         x = _pair_to_f32(self.x0)

@@ -359,59 +359,6 @@ def test_conv_7x1_folded_heads(cuda, split):
     assert d < 2e-4
 
 
-@pytest.mark.parametrize("variant", ["plain", "res_warp"])
-@pytest.mark.parametrize("split", [1, 2])
-def test_conv_fused_instance_norm(cuda, split, variant, monkeypatch):
-    """lwb_conv_plan_fuse_norm against conv + lwb_norm_act_nhwc on the same operands: 512 -> 512 @32x32, batch 3 (24 tiles per
-    N tile: several CTAs wait on every unit), twice in a row (counters / statistics re-zeroed)."""
-    n, c, h, w = 3, 512, 32, 32
-    x = rnd(n, c, h, w, seed=41)
-    wt = rnd(c, c, 3, 3, seed=42, scale=0.03)
-    gamma, beta = (1 + 0.1 * rnd(c, seed=43)).to(cuda), (0.1 * rnd(c, seed=44)).to(cuda)
-    if int(split) == 2:
-        xs = to_f8_operands(cuda, x)
-    else:
-        xs = K.nchw_to_nhwc_split(x.to(cuda), split=True)
-    ws = K.pack_conv_weight(wt.to(cuda), split=split)
-    d = K.make_conv_desc(n, h, w, c, c, 3, 3, stride=1, pad=1, split=split)
-    lo_format = 1 if int(split) == 2 else 0
-    res = rnd(n, h, w, c, seed=45).to(cuda) if variant == "res_warp" else None
-    src = rnd(1, h, w, c, seed=46).to(cuda) if variant == "res_warp" else None
-    T = (torch.rand(n, 64, 64, 2, generator=torch.Generator().manual_seed(47)) * 2.4 - 1.2).to(cuda) if variant == "res_warp" else None
-
-    def outs():
-        return (torch.empty(n, h, w, c, device=cuda), torch.empty(n, h, w, c, dtype=torch.float16, device=cuda),
-                torch.empty(n, h, w, c, dtype=torch.float16, device=cuda))
-    # separate pass
-    raw = torch.empty(n, h, w, c, device=cuda)
-    st = torch.zeros(n, c, 2, dtype=torch.float64, device=cuda)
-    K.ConvPlan(d, xs, None, ws, raw, st).run()
-    y0, hi0, lo0 = outs()
-    wsb = torch.empty(n, c, 2, device=cuda)
-    K.norm_act_nhwc(raw, st, gamma, beta, variant == "plain", wsb, residual=res, warp_src=src, T=T, align_corners=True,
-                    y_f32=y0, y_hi=hi0, y_lo=lo0, lo_format=lo_format)
-    # fused
-    st1 = torch.zeros(n, c, 2, dtype=torch.float64, device=cuda)
-    ctr = torch.zeros(n * 4, dtype=torch.int32, device=cuda)
-    raw1 = torch.full((n, h, w, c), float("nan"), device=cuda)
-    plan = K.ConvPlan(d, xs, None, ws, raw1, st1)
-    y1, hi1, lo1 = outs()
-    ok = plan.fuse_norm(gamma, beta, variant == "plain", ctr, residual=res, warp_src=src, T=T, align_corners=True,
-                        y_f32=y1, y_hi=hi1, y_lo=lo1, lo_format=lo_format)
-    assert ok, "a 32x32 split-mode plan must be fusable"
-    for _ in range(2):
-        st1.zero_()
-        ctr.zero_()
-        plan.run()
-    torch.cuda.synchronize()
-    dy = (y1 - y0).abs().max().item()
-    print("fused norm %s split %d: y max-abs diff %.3e (scale %.2f)" % (variant, split, dy, y0.abs().max().item()))
-    assert dy < 1e-5
-    assert (hi1.float() - hi0.float()).abs().max().item() < 2e-3
-    assert float(lo1.view(torch.uint8).ne(lo0.view(torch.uint8)).float().mean()) < 0.01
-    assert int(ctr[:n * 2].max()) == 8 and int(ctr[:n * 2].min()) == 8          # every unit saw its 8 tiles
-
-
 @pytest.mark.parametrize("split", [1, 2])
 @pytest.mark.parametrize("cin,cout,h", [(128, 64, 32), (256, 128, 24)])
 def test_conv_transposed_merged_phases(cuda, split, cin, cout, h):
