@@ -39,9 +39,9 @@ SIGNATURES = {
     "lwb_correspond": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _f, _vp, _i, _vp, _vp, _i, _i,
                             _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lwb_warp_nchw": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _i, _vp]),
-    "lwb_pack_conv_weight": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "lwb_pack_conv_weight": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "lwb_pack_conv_weight_f8": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
-    "lwb_pack_conv_weight_rowk": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "lwb_pack_conv_weight_rowk": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "lwb_nchw_to_nhwc_split": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "lwb_nhwc_to_nchw": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "lwb_conv_plan_create": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,

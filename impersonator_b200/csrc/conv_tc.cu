@@ -92,7 +92,7 @@ struct ConvParams {
     float* out; int out_h, out_w, cout;
     int oy_mul, oy_add, ox_mul, ox_add;
     double* stats;
-    float out_scale;                  // accumulator -> output (2^-w_exp in f8 mode, else 1)
+    float out_scale;                  // accumulator -> output (2^-w_exp)
     int phase_cols;                   // > 0: merged transposed conv -- column block col / phase_cols = sub-pixel phase (a, b) =
                                       // (ph >> 1, ph & 1) of output pixel (2y + a, 2x + b), channel = col % phase_cols
 };
@@ -717,7 +717,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     LWB_CHECK_ARG(!f8 || (!d->rowk && !d->halo), "the fp8 lo mode is not available for row-K / halo plans");
     LWB_CHECK_ARG(d->n > 0 && d->h_in > 0 && d->w_in > 0 && d->cout > 0, "non-positive size");
     LWB_CHECK_ARG(d->cout % 16 == 0, "cout must be a multiple of 16");
-    LWB_CHECK_ARG(!f8 || (d->w_exp >= -40 && d->w_exp <= 60), "w_exp out of range");
+    LWB_CHECK_ARG(d->w_exp >= -40 && d->w_exp <= 60, "w_exp out of range");
     int n_tile = pick_n_tile(d->cout, d->n_tile);
     LWB_CHECK_ARG(n_tile > 0 && d->cout % n_tile == 0, "no N tile divides cout");
     if (d->halo) {
@@ -742,7 +742,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
         p.n_tiles_n = d->cout / n_tile;
         p.out = out_raw; p.out_h = d->h_out; p.out_w = d->w_out; p.cout = d->cout;
         p.stats = stats;
-        p.out_scale = f8 ? ldexpf(1.f, -d->w_exp) : 1.f;      // weights are packed x 2^w_exp in f8 mode (lwb_pack_conv_weight_f8)
+        p.out_scale = ldexpf(1.f, -d->w_exp);      // weights are packed x 2^w_exp in every operand mode (lwb_pack_conv_weight*)
         L.n_tile = n_tile; L.mode = d->split;
         pick_rings(p, n_tile, split);
         const long total = (long)p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;

@@ -13,10 +13,11 @@ namespace {
 using lwb::split_half;
 
 // ---------------------------------------------------------------------------------------------
-// weights: OIHW (Conv2d) / IOHW (ConvTranspose2d) fp32 -> [tap][cout_pad][cin_pad] fp16 hi/lo
+// weights: OIHW (Conv2d) / IOHW (ConvTranspose2d) fp32 -> [tap][cout_pad][cin_pad] fp16 hi/lo of w * 2^E
+// (wscale = 2^E, the layer's exponent: max|w| * 2^E in [2^14, 2^15) keeps hi and lo out of the fp16 subnormals)
 // ---------------------------------------------------------------------------------------------
 __global__ void k_pack_weight(const float* __restrict__ w, int cout, int cin, int kh, int kw, int transposed,
-                              int cout_pad, int cin_pad, __half* __restrict__ hi, __half* __restrict__ lo)
+                              int cout_pad, int cin_pad, float wscale, __half* __restrict__ hi, __half* __restrict__ lo)
 {
     const long total = (long)kh * kw * cout_pad * cin_pad;
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -30,7 +31,7 @@ __global__ void k_pack_weight(const float* __restrict__ w, int cout, int cin, in
                            : w[(((size_t)co * cin + ci) * kh + ky) * kw + kx];
         }
         __half h, l;
-        split_half(v, h, l);
+        split_half(v * wscale, h, l);
         hi[i] = h;
         if (lo) lo[i] = l;
     }
@@ -78,9 +79,9 @@ __global__ void k_pack_weight_f8(const float* __restrict__ w, int cout, int cin,
 }
 
 // First-layer packing for the row-contiguous 7x7 trick (see conv_tc.cu): [ky][cout_pad][kxs*cpx]
-// with K index = kx*cpx + c  (kx < kw real taps, the rest zero).
+// with K index = kx*cpx + c  (kx < kw real taps, the rest zero), of w * 2^E like k_pack_weight.
 __global__ void k_pack_weight_rowk(const float* __restrict__ w, int cout, int cin, int kh, int kw,
-                                   int cout_pad, int cpx, int kxs, __half* __restrict__ hi, __half* __restrict__ lo)
+                                   int cout_pad, int cpx, int kxs, float wscale, __half* __restrict__ hi, __half* __restrict__ lo)
 {
     const int kk = kxs * cpx;
     const long total = (long)kh * cout_pad * kk;
@@ -92,7 +93,7 @@ __global__ void k_pack_weight_rowk(const float* __restrict__ w, int cout, int ci
         float v = 0.f;
         if (kx < kw && c < cin && co < cout) v = w[(((size_t)co * cin + c) * kh + ky) * kw + kx];
         __half h, l;
-        split_half(v, h, l);
+        split_half(v * wscale, h, l);
         hi[i] = h;
         if (lo) lo[i] = l;
     }
@@ -477,13 +478,14 @@ extern "C" int lwb_gated_bn_nchw(const float* ab, int n, int c, int h, int w, in
 }
 
 extern "C" int lwb_pack_conv_weight(const float* w, int cout, int cin, int kh, int kw, int transposed,
-                                    int cout_pad, int cin_pad, uint16_t* w_hi, uint16_t* w_lo, lwb_stream_t stream)
+                                    int cout_pad, int cin_pad, int w_exp, uint16_t* w_hi, uint16_t* w_lo, lwb_stream_t stream)
 {
     LWB_CHECK_ARG(w && w_hi, "null pointer");
     LWB_CHECK_ARG(cout > 0 && cin > 0 && kh > 0 && kw > 0 && cout_pad >= cout && cin_pad >= cin, "bad sizes");
+    LWB_CHECK_ARG(w_exp >= -40 && w_exp <= 60, "w_exp out of range");
     const long total = (long)kh * kw * cout_pad * cin_pad;
     k_pack_weight<<<(int)min((total + 255) / 256, 4096l), 256, 0, (cudaStream_t)stream>>>(
-        w, cout, cin, kh, kw, transposed, cout_pad, cin_pad, (__half*)w_hi, (__half*)w_lo);
+        w, cout, cin, kh, kw, transposed, cout_pad, cin_pad, ldexpf(1.f, w_exp), (__half*)w_hi, (__half*)w_lo);
     LWB_LAUNCH_OK();
     return LWB_OK;
 }
@@ -502,13 +504,15 @@ extern "C" int lwb_pack_conv_weight_f8(const float* w, int cout, int cin, int kh
 }
 
 extern "C" int lwb_pack_conv_weight_rowk(const float* w, int cout, int cin, int kh, int kw,
-                                         int cout_pad, int cpx, int kxs, uint16_t* w_hi, uint16_t* w_lo, lwb_stream_t stream)
+                                         int cout_pad, int cpx, int kxs, int w_exp, uint16_t* w_hi, uint16_t* w_lo,
+                                         lwb_stream_t stream)
 {
     LWB_CHECK_ARG(w && w_hi, "null pointer");
     LWB_CHECK_ARG(cout > 0 && cin > 0 && cin <= cpx && kw <= kxs && cout_pad >= cout, "bad sizes");
+    LWB_CHECK_ARG(w_exp >= -40 && w_exp <= 60, "w_exp out of range");
     const long total = (long)kh * cout_pad * kxs * cpx;
     k_pack_weight_rowk<<<(int)min((total + 255) / 256, 4096l), 256, 0, (cudaStream_t)stream>>>(
-        w, cout, cin, kh, kw, cout_pad, cpx, kxs, (__half*)w_hi, (__half*)w_lo);
+        w, cout, cin, kh, kw, cout_pad, cpx, kxs, ldexpf(1.f, w_exp), (__half*)w_hi, (__half*)w_lo);
     LWB_LAUNCH_OK();
     return LWB_OK;
 }

@@ -315,9 +315,8 @@ class _StreamBase(object):
         self.ws = torch.empty((self.B, cmax, 2), dtype=torch.float32, device=self.dev)
         pend = [L for L in self._layers if L.wsrc is not None]
         if pend:
-            amax = [None] * len(pend)
-            if self.split == 2:                         # per-layer weight exponent of the fp16f8 packing: ONE host sync
-                amax = torch.stack([L.wsrc[0].abs().max().float() for L in pend]).tolist()
+            # per-layer weight exponent of the packing (kernels.weight_exponent): ONE host sync
+            amax = torch.stack([L.wsrc[0].abs().max().float() for L in pend]).tolist()
             for L, a in zip(pend, amax):
                 L.w = K.pack_conv_weight(L.wsrc[0], transposed=L.wsrc[1], split=self.split, absmax=a)
                 L.wsrc = None

@@ -178,9 +178,7 @@ class _HmrStream(object):
         self.final = x_f32
         self.post_ss = _bn_affine(r.post_bn)
         # weights: one max|w| sync for the whole encoder, then the plans
-        amax = [None] * len(pend)
-        if split == 2:
-            amax = torch.stack([p["w"].abs().max().float() for p in pend]).tolist()
+        amax = torch.stack([p["w"].abs().max().float() for p in pend]).tolist()
         self.plans = []
         for p, a in zip(pend, amax):
             wp = K.pack_conv_weight(p["w"], split=split, absmax=a)

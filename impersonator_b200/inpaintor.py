@@ -252,9 +252,7 @@ class _InpaintStream(object):
         self.att_act = _Act((B, h, w, 128), dev, split)
         self.upsample, h, w = self._chain(list(net.refine_upsample_net), self.att_act, h, w, final_f32=True)
         # one max|w| sync for the whole network, then pack + plan
-        amax = [None] * len(self._pend)
-        if split == 2:
-            amax = torch.stack([p["w"].abs().max().float() for p in self._pend]).tolist()
+        amax = torch.stack([p["w"].abs().max().float() for p in self._pend]).tolist()
         for p, a in zip(self._pend, amax):
             wp = K.pack_conv_weight(p["w"], cout_pad=p["cout_pad"], cin_pad=p["cin_pad"], split=split, absmax=a)
             p["plan"] = K.ConvPlan(p["desc"], p["x"], None, wp, p["raw"], None)

@@ -166,17 +166,17 @@ def warp_nchw(x, T, align_corners=None, out=None, accumulate=False):
 
 
 class PackedWeight(tuple):
-    """(hi, lo) operand tensors of one conv layer; ``w_exp`` = the power of two they were packed with (split = 2)."""
-    w_exp = 15
+    """(hi, lo) operand tensors of one conv layer; ``w_exp`` = the power of two they were packed with (every split)."""
 
-    def __new__(cls, hi, lo, w_exp=15):
+    def __new__(cls, hi, lo, w_exp):
         self = super(PackedWeight, cls).__new__(cls, (hi, lo))
         self.w_exp = w_exp
         return self
 
 
 def weight_exponent(absmax):
-    """Per-layer scale of the fp16f8 weight packing: E with absmax * 2^E in [2^14, 2^15) (15 for an all-zero layer)."""
+    """Per-layer scale of the weight packing in every operand mode: E with absmax * 2^E in [2^14, 2^15) (15 for an
+    all-zero layer).  It keeps the fp16 hi / lo weights of small-weight layers out of the fp16 subnormals."""
     import math
     absmax = float(absmax)
     if not (absmax > 0.0) or math.isinf(absmax) or math.isnan(absmax):
@@ -185,9 +185,9 @@ def weight_exponent(absmax):
 
 
 def pack_conv_weight(w, transposed=False, cout_pad=None, cin_pad=None, split=True, absmax=None):
-    """OIHW / IOHW fp32 -> ([tap][cout_pad][cin_pad] fp16 hi, lo).  split: 0/False single, 1/True fp16 hi+lo,
-    2 fp16 hi (x 2^w_exp) + fp8 pair blocks (lwb_pack_conv_weight_f8).  ``absmax`` = max|w| when the caller already
-    knows it (one host sync per network instead of one per layer); computed here otherwise."""
+    """OIHW / IOHW fp32 -> ([tap][cout_pad][cin_pad] fp16 hi, lo) of w x 2^w_exp.  split: 0/False single, 1/True fp16
+    hi+lo, 2 fp16 hi + fp8 pair blocks (lwb_pack_conv_weight_f8).  ``absmax`` = max|w| when the caller already knows it
+    (one host sync per network instead of one per layer); computed here otherwise."""
     _chk_cuda(w)
     if int(split) == 2:
         return _pack_conv_weight_f8(w, transposed, cout_pad, cin_pad, absmax)
@@ -198,11 +198,12 @@ def pack_conv_weight(w, transposed=False, cout_pad=None, cin_pad=None, split=Tru
         cout, cin, kh, kw = w.shape
     cout_pad = cout_pad or cout
     cin_pad = cin_pad or cin
+    w_exp = weight_exponent(w.abs().max() if absmax is None else absmax)
     hi = torch.empty((kh * kw, cout_pad, cin_pad), dtype=torch.float16, device=w.device)
     lo = torch.empty_like(hi) if split else None
-    check(lib().lwb_pack_conv_weight(ptr(w), cout, cin, kh, kw, 1 if transposed else 0, cout_pad, cin_pad,
+    check(lib().lwb_pack_conv_weight(ptr(w), cout, cin, kh, kw, 1 if transposed else 0, cout_pad, cin_pad, w_exp,
                                      ptr(hi), ptr(lo), stream()), "lwb_pack_conv_weight")
-    return PackedWeight(hi, lo)
+    return PackedWeight(hi, lo, w_exp)
 
 
 def _pack_conv_weight_f8(w, transposed, cout_pad, cin_pad, absmax=None):
@@ -221,17 +222,18 @@ def _pack_conv_weight_f8(w, transposed, cout_pad, cin_pad, absmax=None):
     return PackedWeight(hi, lo, w_exp)
 
 
-def pack_conv_weight_rowk(w, cout_pad=None, cpx=8, kxs=8, split=True):
-    """7x7 stem weights -> [ky][cout_pad][kxs*cpx] fp16 hi, lo (K index = kx*cpx + c)."""
+def pack_conv_weight_rowk(w, cout_pad=None, cpx=8, kxs=8, split=True, absmax=None):
+    """7x7 stem weights -> [ky][cout_pad][kxs*cpx] fp16 hi, lo of w x 2^w_exp (K index = kx*cpx + c)."""
     _chk_cuda(w)
     w = w.float().contiguous()
     cout, cin, kh, kw = w.shape
     cout_pad = cout_pad or cout
+    w_exp = weight_exponent(w.abs().max() if absmax is None else absmax)
     hi = torch.empty((kh, cout_pad, kxs * cpx), dtype=torch.float16, device=w.device)
     lo = torch.empty_like(hi) if split else None
-    check(lib().lwb_pack_conv_weight_rowk(ptr(w), cout, cin, kh, kw, cout_pad, cpx, kxs, ptr(hi), ptr(lo), stream()),
-          "lwb_pack_conv_weight_rowk")
-    return PackedWeight(hi, lo)
+    check(lib().lwb_pack_conv_weight_rowk(ptr(w), cout, cin, kh, kw, cout_pad, cpx, kxs, w_exp, ptr(hi), ptr(lo),
+                                          stream()), "lwb_pack_conv_weight_rowk")
+    return PackedWeight(hi, lo, w_exp)
 
 
 def nchw_to_nhwc_split(x, c_pad=None, pad_hw=(0, 0, 0, 0), hi=None, lo=None, split=True):
@@ -265,11 +267,11 @@ class ConvPlan(object):
     """One conv layer bound to fixed buffers (lwb_conv_plan): build once, run every step."""
 
     def __init__(self, desc, x0, x1, w, out_raw, stats):
-        """x0 / x1 / w: (hi, lo) tensor pairs (x1 may be None); out_raw fp32 NHWC; stats f64 [n,cout,2] or None."""
+        """x0 / x1 / w: (hi, lo) tensor pairs (x1 may be None), w a PackedWeight; out_raw fp32 NHWC; stats f64
+        [n,cout,2] or None."""
         self._keep = (x0, x1, w, out_raw, stats)
         self.desc = desc
-        if desc.split == 2:
-            desc.w_exp = int(getattr(w, "w_exp", 15))
+        desc.w_exp = int(w.w_exp)
         handle = ctypes.c_void_p()
         x1 = x1 or (None, None)
         check(lib().lwb_conv_plan_create(ctypes.byref(desc), ptr(x0[0]), ptr(x0[1]), ptr(x1[0]), ptr(x1[1]),

@@ -101,9 +101,12 @@ int lwb_warp_nchw(const float* x, int src_batch, int channels, int h, int w,
  * ------------------------------------------------------------------------------------------ */
 
 /* Repack an OIHW (Conv2d) or IOHW (ConvTranspose2d, transposed != 0) fp32 weight into the
- * engine's [tap][Cout_pad][Cin_pad] fp16 hi/lo layout (done once at load time). w_lo nullable. */
+ * engine's [tap][Cout_pad][Cin_pad] fp16 hi/lo layout (done once at load time): w_hi = fp16(w * 2^w_exp),
+ * w_lo = fp16(w * 2^w_exp - w_hi).  w_lo nullable.  The caller picks w_exp as for lwb_pack_conv_weight_f8 (max|w| * 2^w_exp
+ * in [2^14, 2^15), so that small weights do not fall into the fp16 subnormals) and passes the same value in
+ * lwb_conv_desc.w_exp; w_exp = 0 packs the weights unscaled. */
 int lwb_pack_conv_weight(const float* w, int cout, int cin, int kh, int kw, int transposed,
-                         int cout_pad, int cin_pad, uint16_t* w_hi, uint16_t* w_lo, lwb_stream_t stream);
+                         int cout_pad, int cin_pad, int w_exp, uint16_t* w_hi, uint16_t* w_lo, lwb_stream_t stream);
 /* Weights for the "fp16 + fp8" operand split (lwb_conv_desc.split = 2): w_hi [taps][cout_pad][cin_pad] fp16 holds
  * fp16(w) * 2^w_exp; w_lo8 (same byte size) holds, per 64-input-channel block of 128 bytes,
  * 64 x e4m3((w - fp16(w)) * 2^(w_exp+4)) followed by 64 x e4m3(w * 2^(w_exp-10)).  The caller picks the layer's w_exp
@@ -112,9 +115,10 @@ int lwb_pack_conv_weight(const float* w, int cout, int cin, int kh, int kw, int 
 int lwb_pack_conv_weight_f8(const float* w, int cout, int cin, int kh, int kw, int transposed,
                             int cout_pad, int cin_pad, int w_exp, uint16_t* w_hi, uint8_t* w_lo8, lwb_stream_t stream);
 
-/* Row-K packing for the 7x7 stem: [ky][cout_pad][kxs*cpx], K index = kx*cpx + c (zero beyond kw / cin). */
+/* Row-K packing for the 7x7 stem: [ky][cout_pad][kxs*cpx], K index = kx*cpx + c (zero beyond kw / cin), hi/lo of
+ * w * 2^w_exp as in lwb_pack_conv_weight. */
 int lwb_pack_conv_weight_rowk(const float* w, int cout, int cin, int kh, int kw,
-                              int cout_pad, int cpx, int kxs, uint16_t* w_hi, uint16_t* w_lo, lwb_stream_t stream);
+                              int cout_pad, int cpx, int kxs, int w_exp, uint16_t* w_hi, uint16_t* w_lo, lwb_stream_t stream);
 
 /* NCHW fp32 -> NHWC fp16 hi/lo [n, hp, wp, c_pad]; input pixel (y,x) lands at (y+oy, x+ox), the rest
  * (spatial border, channels >= c) is zero.  hp >= h+oy, wp >= w+ox.  lo nullable. */
@@ -142,7 +146,8 @@ typedef struct lwb_conv_desc {
     int n_tile;               /* 0 = auto; else force the N tile (16/32/64/128, must divide cout; 256 runs as 128) */
     int halo;                 /* 1 = halo plan (stride-1 'same' k x k convs and the row-K stem): checked as such, then run
                                  by the same tap-group kernel as halo = 0 */
-    int w_exp;                /* split = 2: the power of two the weights were packed with (lwb_pack_conv_weight_f8) */
+    int w_exp;                /* the power of two the weights were packed with (lwb_pack_conv_weight*), every split; the
+                                 output is scaled by 2^-w_exp.  In [-40, 60] */
     int pad_w;                /* horizontal padding when it differs from pad (e.g. a 7x1 filter); -1 = same as pad */
 } lwb_conv_desc;
 

@@ -50,7 +50,7 @@ def pack_conv_weight(w, transposed=False, cout_pad=None, cin_pad=None, split=Tru
     return pw
 
 
-def pack_conv_weight_rowk(w, cout_pad=None, cpx=8, kxs=8, split=True):
+def pack_conv_weight_rowk(w, cout_pad=None, cpx=8, kxs=8, split=True, absmax=None):
     pw = PackedWeight((w.detach().float(), "rowk"))
     pw.w_exp = 15
     return pw

@@ -1,13 +1,13 @@
-"""GPU parity of the conv engine (wgmma implicit GEMM) and its glue kernels against plain
-torch fp32 ops on CPU (the same ATen ops the reference's nn.Conv2d / ConvTranspose2d /
-InstanceNorm2d / grid_sample calls resolve to).  Tolerances: split (parity) mode 2e-4 of the
-output scale; single-pass fp16 ("fast") mode 2e-2."""
-import numpy as np
+"""GPU parity of the conv engine (wgmma implicit GEMM) and its glue kernels.  Every conv result is checked by
+conv_emulation.check_conv: against a float64 emulation of its operand mode's own arithmetic (3e-5 of the output scale),
+against plain torch fp32 on CPU (the same ATen ops the reference's nn.Conv2d / ConvTranspose2d call resolve to: 2e-4 for
+fp16x3, 3e-4 for fp16f8, 2e-2 for single-pass fp16), and its InstanceNorm statistics against the sums of its own output."""
 import pytest
 import torch
 import torch.nn.functional as F
 
 from impersonator_b200 import kernels as K
+from conv_emulation import check_conv, emulate_f8, report  # noqa: F401  (report, emulate_f8: used by the other conv tests)
 
 pytestmark = pytest.mark.gpu
 
@@ -17,19 +17,10 @@ def rnd(*shape, seed=0, scale=1.0):
     return torch.randn(*shape, generator=g) * scale
 
 
-def report(name, got, ref):
-    d = (got - ref).abs()
-    scale = ref.abs().max().item() + 1e-12
-    idx = np.unravel_index(int(d.argmax()), d.shape)
-    print("%s: max-abs %.3e (ref scale %.3e, rel %.3e) at %s; mean-abs %.3e; nonfinite %d"
-          % (name, d.max().item(), scale, d.max().item() / scale, idx, d.mean().item(),
-             int((~torch.isfinite(got)).sum())))
-    return d.max().item() / scale
-
-
 def run_conv(cuda, x, w, stride=1, pad=1, dil=1, transposed=False, split=True, x1=None, n_tile=0, stats=True, halo=False,
-             pad_w=None):
-    """x [n,c,h,w] fp32 CPU, w OIHW (or IOHW when transposed) -> NCHW fp32 CPU result, stats."""
+             pad_w=None, out=None, st=None):
+    """x [n,c,h,w] fp32 CPU, w OIHW (or IOHW when transposed) -> (NCHW fp32 CPU result, stats, the weights' w_exp).
+    ``out`` / ``st``: caller-allocated NHWC output and statistics buffers (NaN- / zero-filled here otherwise)."""
     n, c0, h, wd = x.shape
     if int(split) == 2:
         xs, x1s = to_f8_operands(cuda, x), (to_f8_operands(cuda, x1) if x1 is not None else None)
@@ -42,12 +33,14 @@ def run_conv(cuda, x, w, stride=1, pad=1, dil=1, transposed=False, split=True, x
     d = K.make_conv_desc(n, h, wd, c0, cout, kh, kw, stride=stride, pad=pad, dil=dil,
                          cin1=0 if x1 is None else x1.shape[1], transposed=transposed, split=split, n_tile=n_tile,
                          halo=halo, pad_w=pad_w)
-    out = torch.full((n, d.h_out, d.w_out, cout), float("nan"), dtype=torch.float32, device=cuda)
-    st = torch.zeros((n, cout, 2), dtype=torch.float64, device=cuda) if stats else None
+    if out is None:
+        out = torch.full((n, d.h_out, d.w_out, cout), float("nan"), dtype=torch.float32, device=cuda)
+    if st is None and stats:
+        st = torch.zeros((n, cout, 2), dtype=torch.float64, device=cuda)
     plan = K.ConvPlan(d, xs, x1s, ws, out, st)
     plan.run()
     torch.cuda.synchronize()
-    return K.nhwc_to_nchw(out).cpu(), (st.cpu() if stats else None)
+    return K.nhwc_to_nchw(out).cpu(), (st.cpu() if st is not None else None), ws.w_exp
 
 
 def to_f8_operands(cuda, x):
@@ -57,33 +50,6 @@ def to_f8_operands(cuda, x):
     lo = torch.empty_like(hi)
     K.norm_act_nhwc(raw, None, None, None, False, None, y_hi=hi, y_lo=lo, lo_format=1)
     return hi, lo
-
-
-def q8(t):
-    return t.clamp(-448, 448).to(torch.float8_e4m3fn).double()
-
-
-def emulate_f8(x, w, conv):
-    """The arithmetic the fp16f8 mode is meant to perform (DESIGN.md section 4), in float64 on the CPU:
-    per-layer weight scale 2^E with max|w| * 2^E in [2^14, 2^15); x8 = e4m3(x / 16), xlo8 = e4m3(x_lo * 2^10),
-    wlo8 = e4m3(w_lo * 2^(E+4)), w8 = e4m3(w * 2^(E-10))."""
-    E = K.weight_exponent(w.abs().max())
-    xh = x.half().double()
-    wh = w.half().double()
-    xl, wl = x.double() - xh, w.double() - wh
-    main = conv(xh, wh)
-    t2 = conv(q8(x / 16), q8((wl * 2.0 ** (E + 4)).float())) / 2.0 ** E
-    t3 = conv(q8((xl * 1024).float()), q8(w * 2.0 ** (E - 10))) / 2.0 ** E
-    return (main + t2 + t3).float()
-
-
-def check_stats(st, ref):
-    s = ref.double().sum(dim=(2, 3))
-    q = (ref.double() ** 2).sum(dim=(2, 3))
-    e1 = ((st[..., 0] - s).abs().max() / (s.abs().max() + 1e-9)).item()
-    e2 = ((st[..., 1] - q).abs().max() / (q.abs().max() + 1e-9)).item()
-    print("stats rel err: sum %.3e sumsq %.3e" % (e1, e2))
-    assert e1 < 1e-3 and e2 < 1e-3
 
 
 CASES = [
@@ -107,12 +73,8 @@ def test_conv2d(cuda, case, split):
     name, n, cin, cout, h, w, k, stride, pad, n_tile = case
     x = rnd(n, cin, h, w, seed=1)
     wt = rnd(cout, cin, k, k, seed=2, scale=0.05)
-    ref = F.conv2d(x, wt, stride=stride, padding=pad)
-    got, st = run_conv(cuda, x, wt, stride=stride, pad=pad, split=split, n_tile=n_tile)
-    rel = report(name + ("/split" if split else "/fast"), got, ref)
-    assert rel < (2e-4 if split else 2e-2)
-    if split:
-        check_stats(st, ref)
+    got, st, e = run_conv(cuda, x, wt, stride=stride, pad=pad, split=split, n_tile=n_tile)
+    check_conv(name, split, got, x, wt, lambda a, b: F.conv2d(a, b, stride=stride, padding=pad), e, st)
 
 
 HALO_CASES = [c for c in CASES if c[7] == 1 and c[6] in (3, 7) and c[8] == c[6] // 2] + [
@@ -130,34 +92,26 @@ def test_conv2d_halo(cuda, case, split):
     name, n, cin, cout, h, w, k, stride, pad, n_tile = case
     x = rnd(n, cin, h, w, seed=31)
     wt = rnd(cout, cin, k, k, seed=32, scale=0.05)
-    ref = F.conv2d(x, wt, stride=1, padding=pad)
-    got, st = run_conv(cuda, x, wt, stride=1, pad=pad, split=split, n_tile=n_tile, halo=True)
-    rel = report(name + "/halo" + ("/split" if split else "/fast"), got, ref)
-    assert rel < (2e-4 if split else 2e-2)
-    if split:
-        check_stats(st, ref)
+    got, st, e = run_conv(cuda, x, wt, stride=1, pad=pad, split=split, n_tile=n_tile, halo=True)
+    check_conv(name + "/halo", split, got, x, wt, lambda a, b: F.conv2d(a, b, padding=pad), e, st)
 
 
 @pytest.mark.parametrize("split", [True, False])
 def test_conv_concat_inputs_halo(cuda, split):
     a, b = rnd(2, 64, 32, 32, seed=5), rnd(2, 128, 32, 32, seed=6)
     wt = rnd(64, 192, 3, 3, seed=7, scale=0.05)
-    ref = F.conv2d(torch.cat([a, b], dim=1), wt, padding=1)
-    got, _ = run_conv(cuda, a, wt, split=split, x1=b, halo=True)
-    assert report("concat/halo", got, ref) < (2e-4 if split else 2e-2)
+    got, st, e = run_conv(cuda, a, wt, split=split, x1=b, halo=True)
+    check_conv("concat/halo", split, got, torch.cat([a, b], dim=1), wt, lambda xx, ww: F.conv2d(xx, ww, padding=1), e, st)
 
 
 @pytest.mark.parametrize("split", [True, False])
 def test_conv_transpose(cuda, split):
+    conv = lambda a, b: F.conv_transpose2d(a, b, stride=2, padding=1, output_padding=1)      # noqa: E731
     for cin, cout, h in ((128, 64, 32), (512, 256, 32)):
         x = rnd(2, cin, h, h, seed=3)
         wt = rnd(cin, cout, 3, 3, seed=4, scale=0.05)
-        ref = F.conv_transpose2d(x, wt, stride=2, padding=1, output_padding=1)
-        got, st = run_conv(cuda, x, wt, stride=2, pad=1, transposed=True, split=split)
-        rel = report("convT_%d_%d" % (cin, cout), got, ref)
-        assert rel < (2e-4 if split else 2e-2)
-        if split:
-            check_stats(st, ref)
+        got, st, e = run_conv(cuda, x, wt, stride=2, pad=1, transposed=True, split=split)
+        check_conv("convT_%d_%d" % (cin, cout), split, got, x, wt, conv, e, st)
 
 
 @pytest.mark.parametrize("split", [True, False])
@@ -165,9 +119,21 @@ def test_conv_concat_inputs(cuda, split):
     """skippers: conv(cat[skip, d]) without materialising the cat (networks/generator.py:177-179)."""
     a, b = rnd(2, 64, 32, 32, seed=5), rnd(2, 128, 32, 32, seed=6)
     wt = rnd(64, 192, 3, 3, seed=7, scale=0.05)
-    ref = F.conv2d(torch.cat([a, b], dim=1), wt, padding=1)
-    got, _ = run_conv(cuda, a, wt, split=split, x1=b)
-    assert report("concat", got, ref) < (2e-4 if split else 2e-2)
+    got, st, e = run_conv(cuda, a, wt, split=split, x1=b)
+    check_conv("concat", split, got, torch.cat([a, b], dim=1), wt, lambda xx, ww: F.conv2d(xx, ww, padding=1), e, st)
+
+
+def run_stem(cuda, x, wt, split, halo=False):
+    """The 7x7 stem (6 -> 64 channels) through the row-K layout: padded NHWC8 input, [ky][cout][kx*8 + c] weights."""
+    n, _, h, w = x.shape
+    xs = K.nchw_to_nhwc_split(x.to(cuda), c_pad=8, pad_hw=(3, 3, 3, 5), split=split)
+    ws = K.pack_conv_weight_rowk(wt.to(cuda), split=split)
+    d = K.make_conv_desc(n, h, w, 8, 64, 7, 7, stride=1, pad=3, split=split, rowk=True, row_pitch=w + 8, halo=halo)
+    out = torch.full((n, h, w, 64), float("nan"), dtype=torch.float32, device=cuda)
+    st = torch.zeros((n, 64, 2), dtype=torch.float64, device=cuda)
+    K.ConvPlan(d, xs, None, ws, out, st).run()
+    torch.cuda.synchronize()
+    return K.nhwc_to_nchw(out).cpu(), st.cpu(), ws.w_exp
 
 
 @pytest.mark.parametrize("halo", [False, True])
@@ -175,21 +141,10 @@ def test_conv_concat_inputs(cuda, split):
 @pytest.mark.parametrize("size", [32, 256])
 def test_stem_7x7_rowk(cuda, split, size, halo):
     """7x7 stem (6 -> 64 channels) through the row-K layout (networks/generator.py:80-84)."""
-    n = 2
-    x = rnd(n, 6, size, size, seed=8)
+    x = rnd(2, 6, size, size, seed=8)
     wt = rnd(64, 6, 7, 7, seed=9, scale=0.05)
-    ref = F.conv2d(x, wt, padding=3)
-    pitch = size + 8
-    xs = K.nchw_to_nhwc_split(x.to(cuda), c_pad=8, pad_hw=(3, 3, 3, 5), split=split)
-    ws = K.pack_conv_weight_rowk(wt.to(cuda), split=split)
-    d = K.make_conv_desc(n, size, size, 8, 64, 7, 7, stride=1, pad=3, split=split, rowk=True, row_pitch=pitch, halo=halo)
-    out = torch.full((n, size, size, 64), float("nan"), dtype=torch.float32, device=cuda)
-    st = torch.zeros((n, 64, 2), dtype=torch.float64, device=cuda)
-    K.ConvPlan(d, xs, None, ws, out, st).run()
-    torch.cuda.synchronize()
-    got = K.nhwc_to_nchw(out).cpu()
-    assert report("stem_rowk_%d" % size, got, ref) < (2e-4 if split else 2e-2)
-    check_stats(st.cpu(), ref)
+    got, st, e = run_stem(cuda, x, wt, split, halo=halo)
+    check_conv("stem_rowk_%d" % size, split, got, x, wt, lambda a, b: F.conv2d(a, b, padding=3), e, st)
 
 
 def test_heads_7x7(cuda):
@@ -268,30 +223,20 @@ def test_conv2d_fp16f8(cuda, case):
     name, n, cin, cout, h, w, k, stride, pad, n_tile = case
     x = rnd(n, cin, h, w, seed=1)
     wt = rnd(cout, cin, k, k, seed=2, scale=0.05)
-    ref = F.conv2d(x, wt, stride=stride, padding=pad)
-    got, st = run_conv(cuda, x, wt, stride=stride, pad=pad, split=2, n_tile=n_tile)
-    rel = report(name + "/fp16f8 vs fp32", got, ref)
-    assert rel < 3e-4
-    emu = emulate_f8(x, wt, lambda a, b: F.conv2d(a, b, stride=stride, padding=pad))
-    rel_e = report(name + "/fp16f8 vs its float64 emulation", got, emu)
-    assert rel_e < 3e-5                      # only the fp32 accumulation order of the 2^15-scaled sums differs
-    check_stats(st, ref)
+    got, st, e = run_conv(cuda, x, wt, stride=stride, pad=pad, split=2, n_tile=n_tile)
+    check_conv(name, 2, got, x, wt, lambda a, b: F.conv2d(a, b, stride=stride, padding=pad), e, st)
 
 
 def test_conv_transposed_and_concat_fp16f8(cuda):
     x = rnd(2, 128, 32, 32, seed=5)
     wt = rnd(128, 64, 3, 3, seed=6, scale=0.05)
-    ref = F.conv_transpose2d(x, wt, stride=2, padding=1, output_padding=1)
-    got, _ = run_conv(cuda, x, wt, stride=2, pad=1, transposed=True, split=2, stats=False)
-    assert report("convT 128->64 /fp16f8", got, ref) < 3e-4
-    emu = emulate_f8(x, wt, lambda a, b: F.conv_transpose2d(a, b, stride=2, padding=1, output_padding=1))
-    assert report("convT 128->64 /fp16f8 vs emulation", got, emu) < 1e-5
+    got, _, e = run_conv(cuda, x, wt, stride=2, pad=1, transposed=True, split=2, stats=False)
+    check_conv("convT 128->64", 2, got, x, wt, lambda a, b: F.conv_transpose2d(a, b, stride=2, padding=1, output_padding=1),
+               e, emu_bar=1e-5)
     a, b = rnd(1, 64, 64, 64, seed=7), rnd(1, 64, 64, 64, seed=8)
     w2 = rnd(64, 128, 3, 3, seed=9, scale=0.05)
-    ref = F.conv2d(torch.cat([a, b], dim=1), w2, padding=1)
-    got, st = run_conv(cuda, a, w2, split=2, x1=b)
-    assert report("concat 64+64->64 /fp16f8", got, ref) < 3e-4
-    check_stats(st, ref)
+    got, st, e = run_conv(cuda, a, w2, split=2, x1=b)
+    check_conv("concat 64+64->64", 2, got, torch.cat([a, b], dim=1), w2, lambda xx, ww: F.conv2d(xx, ww, padding=1), e, st)
 
 
 @pytest.mark.parametrize("split", [1, 2])
@@ -302,8 +247,8 @@ def test_conv_homogeneity_and_batch_invariance_at_full_batch(cuda, split):
     x1 = rnd(1, 512, 32, 32, seed=3)
     x = x1.expand(16, -1, -1, -1).contiguous()
     wt = rnd(512, 512, 3, 3, seed=4, scale=0.02)
-    y, _ = run_conv(cuda, x, wt, split=split, stats=False)
-    y2, _ = run_conv(cuda, 2 * x, wt, split=split, stats=False)
+    y, _, _ = run_conv(cuda, x, wt, split=split, stats=False)
+    y2, _, _ = run_conv(cuda, 2 * x, wt, split=split, stats=False)
     assert report("conv(2x) vs 2 conv(x)", y2, 2 * y) < 2e-5
     assert torch.equal(y[0], y[15]) and torch.equal(y[0], y[7])
     ref = F.conv2d(x1, wt, padding=1)
@@ -333,23 +278,22 @@ def test_conv2d_round2_shapes(cuda, case, split):
     name, n, cin, cout, h, w, k, stride, pad, dil, n_tile = case
     x = rnd(n, cin, h, w, seed=11)
     wt = rnd(cout, cin, k, k, seed=12, scale=0.05)
-    ref = F.conv2d(x, wt, stride=stride, padding=pad, dilation=dil)
-    got, st = run_conv(cuda, x, wt, stride=stride, pad=pad, dil=dil, split=split, n_tile=n_tile)
-    rel = report(name + "/split%d" % split, got, ref)
-    assert rel < 3e-4
-    check_stats(st, ref)
+    got, st, e = run_conv(cuda, x, wt, stride=stride, pad=pad, dil=dil, split=split, n_tile=n_tile)
+    check_conv(name, split, got, x, wt, lambda a, b: F.conv2d(a, b, stride=stride, padding=pad, dilation=dil), e, st)
 
 
 @pytest.mark.parametrize("split", [1, 2])
 def test_conv_7x1_folded_heads(cuda, split):
     """The 7x7 heads as a 7x1 filter with N = 7 columns x 4 channels (generator.fold_head_weights) + the column sum in
-    lwb_heads_composite(folded_kw=7), against F.conv2d + tanh / sigmoid."""
+    lwb_heads_composite(folded_kw=7): the raw plan output against the emulation of the 7x1 conv, the composite against
+    F.conv2d + tanh / sigmoid."""
     from impersonator_b200.generator import fold_head_weights
     n, h, w = 2, 48, 40
     x = rnd(n, 64, h, w, seed=21)
     w_img, w_att = rnd(3, 64, 7, 7, seed=22, scale=0.02), rnd(1, 64, 7, 7, seed=23, scale=0.02)
     folded = fold_head_weights(w_img, w_att)
-    raw, _ = run_conv(cuda, x, folded, stride=1, pad=3, pad_w=0, split=split, n_tile=32, stats=False)
+    raw, _, e = run_conv(cuda, x, folded, stride=1, pad=3, pad_w=0, split=split, n_tile=32, stats=False)
+    check_conv("folded 7x1 raw", split, raw, x, folded, lambda a, b: F.conv2d(a, b, padding=(3, 0)), e)
     raw_nhwc = raw.permute(0, 2, 3, 1).contiguous().to(cuda)
     color, mask, _ = K.heads_composite(raw_nhwc, None, folded_kw=7)
     ref_c = torch.tanh(F.conv2d(x, w_img, padding=3))
@@ -359,26 +303,33 @@ def test_conv_7x1_folded_heads(cuda, split):
     assert d < 2e-4
 
 
-@pytest.mark.parametrize("split", [1, 2])
-@pytest.mark.parametrize("cin,cout,h", [(128, 64, 32), (256, 128, 24)])
-def test_conv_transposed_merged_phases(cuda, split, cin, cout, h):
-    """lwb_conv_desc.transposed = 2: ConvTranspose2d(k3, s2, p1, op1) as ONE stride-1 pass with the four sub-pixel phases
-    stacked on N (generator.merge_transposed_weight), against F.conv_transpose2d; statistics shared by the four phases."""
+def run_merged_transposed(cuda, x, wt, split, out=None, st=None):
+    """ConvTranspose2d(k3, s2, p1, op1) as one merged-phase plan (lwb_conv_desc.transposed = 2)."""
     from impersonator_b200.generator import merge_transposed_weight
-    n, w = 2, 40
-    x = rnd(n, cin, h, w, seed=51)
-    wt = rnd(cin, cout, 3, 3, seed=52, scale=0.05)
-    ref = F.conv_transpose2d(x, wt, stride=2, padding=1, output_padding=1)
-    xs = to_f8_operands(cuda, x) if split == 2 else K.nchw_to_nhwc_split(x.to(cuda), split=True)
+    n, cin, h, w = x.shape
+    cout = wt.shape[1]
+    xs = to_f8_operands(cuda, x) if split == 2 else K.nchw_to_nhwc_split(x.to(cuda), split=split)
     ws = K.pack_conv_weight(merge_transposed_weight(wt.to(cuda)), split=split)
     d = K.make_conv_desc(n, h, w, cin, cout, 3, 3, stride=2, pad=1, transposed=True, split=split)
     d.transposed = 2
-    out = torch.full((n, 2 * h, 2 * w, cout), float("nan"), device=cuda)
-    st = torch.zeros(n, cout, 2, dtype=torch.float64, device=cuda)
+    if out is None:
+        out = torch.full((n, 2 * h, 2 * w, cout), float("nan"), device=cuda)
+    if st is None:
+        st = torch.zeros(n, cout, 2, dtype=torch.float64, device=cuda)
     plan = K.ConvPlan(d, xs, None, ws, out, st)
     assert plan.num_launches == 1
     plan.run()
     torch.cuda.synchronize()
-    got = K.nhwc_to_nchw(out).cpu()
-    assert report("merged convT %d->%d split %d" % (cin, cout, split), got, ref) < 3e-4
-    check_stats(st.cpu(), ref)
+    return K.nhwc_to_nchw(out).cpu(), st.cpu(), ws.w_exp
+
+
+@pytest.mark.parametrize("split", [1, 2, 0])
+@pytest.mark.parametrize("cin,cout,h", [(128, 64, 32), (256, 128, 24)])
+def test_conv_transposed_merged_phases(cuda, split, cin, cout, h):
+    """lwb_conv_desc.transposed = 2: ConvTranspose2d(k3, s2, p1, op1) as ONE stride-1 pass with the four sub-pixel phases
+    stacked on N (generator.merge_transposed_weight), against F.conv_transpose2d; statistics shared by the four phases."""
+    x = rnd(2, cin, h, 40, seed=51)
+    wt = rnd(cin, cout, 3, 3, seed=52, scale=0.05)
+    got, st, e = run_merged_transposed(cuda, x, wt, split)
+    check_conv("merged convT %d->%d" % (cin, cout), split, got, x, wt,
+               lambda a, b: F.conv_transpose2d(a, b, stride=2, padding=1, output_padding=1), e, st)

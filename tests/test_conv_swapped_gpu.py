@@ -7,26 +7,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from impersonator_b200 import kernels as K
-from test_conv_gpu import check_stats, emulate_f8, report, rnd, run_conv
+from conv_emulation import check_conv
+from test_conv_gpu import rnd, run_conv, run_stem
 
 pytestmark = pytest.mark.gpu
 
 SPLITS = [2, 1, 0]
-
-
-def check(name, split, got, x, wt, conv, st=None):
-    ref = conv(x, wt)
-    if split == 2:
-        assert report(name + "/f8 vs fp32", got, ref) < 3e-4
-        # the fp16f8 arithmetic itself, emulated in float64: only the fp32 summation order differs
-        assert report(name + "/f8", got, emulate_f8(x, wt, conv)) < 3e-5
-    elif split == 1:
-        assert report(name + "/x3", got, ref) < 2e-4
-    else:
-        assert report(name + "/fp16", got, ref) < 2e-2
-    if st is not None and split:
-        check_stats(st, ref)
 
 
 CASES = [
@@ -45,18 +31,18 @@ def test_conv_swapped(cuda, case, split):
     x = rnd(n, cin, h, w, seed=61)
     wt = rnd(cout, cin, k, k, seed=62, scale=0.05)
     conv = lambda a, b: F.conv2d(a, b, stride=stride, padding=k // 2)      # noqa: E731
-    got, st = run_conv(cuda, x, wt, stride=stride, pad=k // 2, split=split, n_tile=n_tile)
-    check(name, split, got, x, wt, conv, st)
+    got, st, e = run_conv(cuda, x, wt, stride=stride, pad=k // 2, split=split, n_tile=n_tile)
+    check_conv(name, split, got, x, wt, conv, e, st)
 
 
-@pytest.mark.parametrize("split", SPLITS)
-def test_conv_swapped_concat(cuda, split):
-    """The 64+64 -> 64 skipper: K chunks from two tensors."""
-    a, b = rnd(2, 64, 40, 24, seed=63), rnd(2, 64, 40, 24, seed=64)
-    wt = rnd(64, 128, 3, 3, seed=65, scale=0.05)
+@pytest.mark.parametrize("split,cin1", [(2, 64), (1, 64), (0, 64), (1, 128)], ids=["2", "1", "0", "1-cin1_128"])
+def test_conv_swapped_concat(cuda, split, cin1):
+    """The 64+64 -> 64 skipper: K chunks from two tensors (and 64+128, where the second tensor has two K chunks)."""
+    a, b = rnd(2, 64, 40, 24, seed=63), rnd(2, cin1, 40, 24, seed=64)
+    wt = rnd(64, 64 + cin1, 3, 3, seed=65, scale=0.05)
     conv = lambda xx, ww: F.conv2d(xx, ww, padding=1)      # noqa: E731
-    got, st = run_conv(cuda, a, wt, split=split, x1=b)
-    check("concat_64_64", split, got, torch.cat([a, b], dim=1), wt, conv, st)
+    got, st, e = run_conv(cuda, a, wt, split=split, x1=b)
+    check_conv("concat_64_%d" % cin1, split, got, torch.cat([a, b], dim=1), wt, conv, e, st)
 
 
 @pytest.mark.parametrize("split", SPLITS)
@@ -65,8 +51,8 @@ def test_conv_swapped_transposed_phases(cuda, split):
     x = rnd(2, 128, 20, 12, seed=66)
     wt = rnd(128, 64, 3, 3, seed=67, scale=0.05)
     conv = lambda a, b: F.conv_transpose2d(a, b, stride=2, padding=1, output_padding=1)      # noqa: E731
-    got, st = run_conv(cuda, x, wt, stride=2, pad=1, transposed=True, split=split)
-    check("convT_128_64", split, got, x, wt, conv, st)
+    got, st, e = run_conv(cuda, x, wt, stride=2, pad=1, transposed=True, split=split)
+    check_conv("convT_128_64", split, got, x, wt, conv, e, st)
 
 
 @pytest.mark.parametrize("split", SPLITS)
@@ -76,8 +62,8 @@ def test_conv_swapped_odd_tiles_many_rounds(cuda, split):
     x = rnd(15, 64, 72, 24, seed=68)
     wt = rnd(64, 64, 3, 3, seed=69, scale=0.05)
     conv = lambda a, b: F.conv2d(a, b, padding=1)      # noqa: E731
-    got, st = run_conv(cuda, x, wt, pad=1, split=split)
-    check("odd_tiles", split, got, x, wt, conv, st)
+    got, st, e = run_conv(cuda, x, wt, pad=1, split=split)
+    check_conv("odd_tiles", split, got, x, wt, conv, e, st)
 
 
 @pytest.mark.parametrize("split", [1, 0])
@@ -85,15 +71,7 @@ def test_conv_swapped_odd_tiles_many_rounds(cuda, split):
 def test_stem_rowk_swapped(cuda, split, size):
     """The 7x7 stem (6 -> 64) through the row-K layout at sizes 32 does not divide (38-row boxes, partial last tile).
     The row-K plan has no fp8 path: fp16x3 is what the generator runs it in."""
-    n = 2
-    x = rnd(n, 6, size, size, seed=70)
+    x = rnd(2, 6, size, size, seed=70)
     wt = rnd(64, 6, 7, 7, seed=71, scale=0.05)
-    xs = K.nchw_to_nhwc_split(x.to(cuda), c_pad=8, pad_hw=(3, 3, 3, 5), split=split)
-    ws = K.pack_conv_weight_rowk(wt.to(cuda), split=split)
-    d = K.make_conv_desc(n, size, size, 8, 64, 7, 7, stride=1, pad=3, split=split, rowk=True, row_pitch=size + 8)
-    out = torch.full((n, size, size, 64), float("nan"), dtype=torch.float32, device=cuda)
-    st = torch.zeros((n, 64, 2), dtype=torch.float64, device=cuda)
-    K.ConvPlan(d, xs, None, ws, out, st).run()
-    torch.cuda.synchronize()
-    got = K.nhwc_to_nchw(out).cpu()
-    check("stem_rowk_%d" % size, split, got, x, wt, lambda a, b: F.conv2d(a, b, padding=3), st.cpu())
+    got, st, e = run_stem(cuda, x, wt, split)
+    check_conv("stem_rowk_%d" % size, split, got, x, wt, lambda a, b: F.conv2d(a, b, padding=3), e, st)

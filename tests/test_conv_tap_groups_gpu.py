@@ -1,10 +1,11 @@
 """Tap-group shapes of the conv engine that the layer tests do not reach: a filter column longer than one y-halo group
 (split into two groups), dilated taps (groups of one) and a 4x4 stride-2 filter (two parity views with two-tap groups),
-in the fp16x3 and fp16f8 operand modes, against torch fp32 on CPU."""
+in the fp16x3 and fp16f8 operand modes, against float64 emulations of their arithmetic and torch fp32 on CPU."""
 import pytest
 import torch.nn.functional as F
 
-from test_conv_gpu import check_stats, emulate_f8, report, rnd, run_conv
+from conv_emulation import check_conv
+from test_conv_gpu import rnd, run_conv
 
 pytestmark = pytest.mark.gpu
 
@@ -24,12 +25,8 @@ def test_conv_tap_groups(cuda, case, split):
     wt = rnd(cout, cin, kh, kw, seed=42, scale=0.05)
     padding = (pad, pad if pad_w is None else pad_w)
     conv = lambda a, b: F.conv2d(a, b, stride=stride, padding=padding, dilation=dil)      # noqa: E731
-    got, _ = run_conv(cuda, x, wt, stride=stride, pad=pad, pad_w=pad_w, dil=dil, split=split)
-    if split == 2:
-        # the fp16f8 arithmetic itself, emulated in float64: only the fp32 summation order differs
-        assert report(name + "/f8", got, emulate_f8(x, wt, conv)) < 3e-5
-    else:
-        assert report(name + "/x3", got, conv(x, wt)) < 2e-4
+    got, st, e = run_conv(cuda, x, wt, stride=stride, pad=pad, pad_w=pad_w, dil=dil, split=split)
+    check_conv(name, split, got, x, wt, conv, e, st)
 
 
 @pytest.mark.parametrize("split", [1, 2])
@@ -39,9 +36,5 @@ def test_conv_odd_m_tiles_many_rounds(cuda, split):
     x = rnd(15, 64, 40, 24, seed=43)
     wt = rnd(256, 64, 3, 3, seed=44, scale=0.05)
     conv = lambda a, b: F.conv2d(a, b, padding=1)      # noqa: E731
-    got, st = run_conv(cuda, x, wt, pad=1, split=split)
-    if split == 2:
-        assert report("odd_m/f8", got, emulate_f8(x, wt, conv)) < 3e-5
-    else:
-        assert report("odd_m/x3", got, conv(x, wt)) < 2e-4
-    check_stats(st, conv(x, wt))
+    got, st, e = run_conv(cuda, x, wt, pad=1, split=split)
+    check_conv("odd_m", split, got, x, wt, conv, e, st)
