@@ -67,6 +67,18 @@ SIGNATURES = {
     "lwb_global_avgpool_nhwc": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _vp]),
     "lwb_linear": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "lwb_conv2d_direct_nchw": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "lwb_det_transform": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "lwb_det_stem_pool": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwb_det_bias_act": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "lwb_det_d2s_bias_relu": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "lwb_det_rpn": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _f, _f, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lwb_det_nms_workspace_bytes": (_sz, [_i, _i]),
+    "lwb_det_nms": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lwb_det_roi_align": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "lwb_det_box_candidates": (_i, [_vp, _i, _i, _vp, _vp, _i, _f, _f, _f, _f, _f, _vp, _vp, _vp, _vp, _vp]),
+    "lwb_det_mask_probs": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "lwb_det_paste_masks": (_i, [_vp, _i, _vp, _vp, _i, _f, _f, _i, _i, _vp, _vp, _vp]),
+    "lwb_det_person_mask": (_i, [_vp, _vp, _vp, _i, _vp, _i, _i, _f, _i, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -17,9 +17,12 @@ warp), one generator pass on the wgmma conv engine, one device->host copy per ch
 results are returned per frame, in order, with ``tsf_info`` describing the last frame.
 
 ``tgt_smpls=None`` (how run_imitator.py:239-241 calls it) sends the target images through the HMR encoder
-(impersonator_b200.hmr, one batch per chunk).  Out of scope (SURVEY.md section 8): ``post_personalize`` (fine-tuning,
-needs backward) and the Mask-RCNN detector.  Any object with ``__call__(img) -> theta`` and ``get_details(theta)``
-can be injected as ``hmr`` (tests use a synthetic body model).
+(impersonator_b200.hmr, one batch per chunk).  ``opt.has_detector`` builds the Mask R-CNN person detector
+(impersonator_b200.detectors, ks = ``opt.bg_ks``; weights from torch's hub cache) and ``personalize`` then takes the
+background mask from its dilated body mask, as models/imitator.py:116-122 does.  Out of scope (SURVEY.md section 8):
+``post_personalize`` (fine-tuning, needs backward).  Any object with ``__call__(img) -> theta`` and
+``get_details(theta)`` can be injected as ``hmr`` (tests use a synthetic body model), and any object with
+``inference(img) -> (bbox, body_mask)`` as ``detector``.
 """
 import os
 
@@ -83,7 +86,7 @@ class Imitator(object):
     asset files.  The keyword arguments are an extension: any of them replaces the corresponding constructed object
     (tests and benchmarks inject synthetic networks / tables because every asset is an external download)."""
 
-    def __init__(self, opt, generator=None, bgnet=None, hmr=None, render=None, device=None):
+    def __init__(self, opt, generator=None, bgnet=None, hmr=None, render=None, device=None, detector=None):
         self._name = 'Imitator'
         self._opt = opt
         self._gpu_ids = getattr(opt, 'gpu_ids', '0')
@@ -91,7 +94,7 @@ class Imitator(object):
         self._save_dir = os.path.join(getattr(opt, 'checkpoints_dir', './outputs/checkpoints/'), getattr(opt, 'name', 'running'))
         self.device = torch.device(device if device is not None else 'cuda')
         self._G_cond_nc, self._D_cond_nc = self.cond_nc()
-        self._create_networks(generator, bgnet, hmr, render)
+        self._create_networks(generator, bgnet, hmr, render, detector)
         self.src_info = None
         self.tsf_info = None
         self.first_cam = None
@@ -111,7 +114,7 @@ class Imitator(object):
         return nc, nc
 
     # ---- construction (models/imitator.py:25-74) -------------------------------------------------
-    def _create_networks(self, generator=None, bgnet=None, hmr=None, render=None):
+    def _create_networks(self, generator=None, bgnet=None, hmr=None, render=None, detector=None):
         opt = self._opt
         self.generator = (generator if generator is not None else self._create_generator()).to(self.device).eval()
         if bgnet is not None:
@@ -128,10 +131,14 @@ class Imitator(object):
             render = SMPLRenderer(image_size=opt.image_size, tex_size=getattr(opt, 'tex_size', 3),
                                   has_front=getattr(opt, 'front_warp', False), fill_back=False)
         self.render = render.to(self.device)
-        if getattr(opt, 'has_detector', False):
-            raise LwbError("has_detector: the Mask-RCNN person detector (utils/detectors.py) is outside the hot path "
-                           "(SURVEY.md section 8); the silhouette-based masks of models/imitator.py:123-125 are used")
-        self.detector = None
+        if detector is not None:
+            self.detector = detector
+        elif getattr(opt, 'has_detector', False):                       # models/imitator.py:43-46
+            from .detectors import PersonMaskRCNNDetector
+            self.detector = PersonMaskRCNNDetector(ks=getattr(opt, 'bg_ks', 13), threshold=0.5, to_gpu=False)
+            self.detector.model = self.detector.model.to(self.device)
+        else:
+            self.detector = None
 
     def _create_bgnet(self):
         from .networks import NetworksFactory
@@ -236,8 +243,12 @@ class Imitator(object):
         src_info['img'] = img
         src_info['image'] = ori_img
 
-        bg_mask = morph(src_info['cond'][:, -1:, :, :], ks=getattr(self._opt, 'bg_ks', 13), mode='erode')
-        body_mask = 1 - bg_mask
+        if self.detector is not None:                                  # models/imitator.py:116-118
+            _, body_mask = self.detector.inference(img[0])
+            bg_mask = 1 - body_mask
+        else:
+            bg_mask = morph(src_info['cond'][:, -1:, :, :], ks=getattr(self._opt, 'bg_ks', 13), mode='erode')
+            body_mask = 1 - bg_mask
         if self.bgnet is self.generator.bg_model:
             bg_inputs = torch.cat([img * bg_mask, bg_mask], dim=1)
             src_info['bg'] = self._original_bg(bg_inputs, self.bgnet(bg_inputs))

@@ -544,3 +544,143 @@ def smpl_forward(beta, theta, model, rotate_base=False, cam=None, want_joints=Tr
         "lwb_smpl_forward")
     _count(3 if want_joints else 2)
     return verts, joints, Rs, Jt, j2d
+
+
+# ---- Mask R-CNN person detector (impersonator_b200.detectors) ------------------------------------------------------
+def _i32_ptrs(values):
+    """Host list of ints -> a C int array for the launchers' host-side const int* arguments."""
+    return (ctypes.c_int * len(values))(*[int(v) for v in values])
+
+
+def det_transform(img, ho, wo, hp, wp, out=None):
+    """[3,h,w] in [-1,1] -> (img + 1) / 2, normalised, bilinear to [ho, wo], zero padded to [1,3,hp,wp]."""
+    _chk_cuda(img, out)
+    _, h, w = img.shape
+    if out is None:
+        out = torch.empty((1, 3, hp, wp), dtype=torch.float32, device=img.device)
+    _count(1)
+    check(lib().lwb_det_transform(ptr(img), h, w, ho, wo, hp, wp, ptr(out), stream()), "lwb_det_transform")
+    return out
+
+
+def det_stem_pool(x, scale, shift, y_hi, y_lo):
+    _chk_cuda(x, scale, shift, y_hi, y_lo)
+    n, c, h, w = x.shape
+    _count(1)
+    check(lib().lwb_det_stem_pool(ptr(x), n, c, h, w, ptr(scale), ptr(shift), ptr(y_hi), ptr(y_lo), stream()), "lwb_det_stem_pool")
+
+
+def det_bias_act(raw, bias=None, relu=False, raw2=None, res=None, res_half=False, step=1, out_hw=None, c=None,
+                 y_f32=None, y_hi=None, y_lo=None):
+    """y = act(raw[step * (y, x)] + raw2 + bias + res) (res nearest-2x upsampled when res_half) -> fp32 / operands."""
+    _chk_cuda(raw, raw2, bias, res, y_f32, y_hi, y_lo)
+    n, h_in, w_in, ld = raw.shape
+    c = c or ld
+    h, w = out_hw or (h_in, w_in)
+    _count(1)
+    with _Prof("det", 0.0):
+        check(lib().lwb_det_bias_act(ptr(raw), ld, ptr(raw2), ptr(bias), ptr(res), 1 if (res_half and res is not None) else 0, int(step), h_in, w_in,
+                                     1 if relu else 0, n, h, w, c, ptr(y_f32), ptr(y_hi), ptr(y_lo), stream()), "lwb_det_bias_act")
+
+
+def det_d2s_bias_relu(raw, bias, y_f32=None, y_hi=None, y_lo=None):
+    _chk_cuda(raw, bias, y_f32, y_hi, y_lo)
+    n, h, w, c4 = raw.shape
+    _count(1)
+    check(lib().lwb_det_d2s_bias_relu(ptr(raw), ptr(bias), n, h, w, c4 // 4, ptr(y_f32), ptr(y_hi), ptr(y_lo), stream()),
+          "lwb_det_d2s_bias_relu")
+
+
+def det_rpn(heads, strides, cell_anchors, bias, k, clip_hw, min_size, xform_clip, out):
+    """heads: list of [gh,gw,16] raw head outputs; out: dict of candidate buffers (boxes, scores, groups, valid, top)."""
+    _chk_cuda(bias, *heads)
+    L = len(heads)
+    offs, o = [], 0
+    for hd in heads:
+        offs.append(o)
+        o += min(k, hd.shape[0] * hd.shape[1] * 3)
+    hp = (ctypes.c_void_p * L)(*[h.data_ptr() for h in heads])
+    cell = cell_anchors.detach().cpu().float().contiguous().numpy()
+    cell_c = (ctypes.c_float * cell.size)(*cell.ravel().tolist())
+    _count(1)
+    check(lib().lwb_det_rpn(L, hp, _i32_ptrs([h.shape[0] for h in heads]), _i32_ptrs([h.shape[1] for h in heads]),
+                            _i32_ptrs([s[0] for s in strides]), _i32_ptrs([s[1] for s in strides]), cell_c,
+                            _i32_ptrs(offs), ptr(bias), int(k), float(clip_hw[0]), float(clip_hw[1]), float(min_size),
+                            float(xform_clip), ptr(out.get("top")), ptr(out["boxes"]), ptr(out["scores"]), ptr(out["groups"]),
+                            ptr(out["valid"]), stream()), "lwb_det_rpn")
+    return o
+
+
+def det_nms(boxes, scores, groups, valid, thresh, max_keep, m_max=None, out=None):
+    """Batched NMS (per group, torchvision's vanilla branch) over n slots -> dict(keep, boxes, scores, groups, count)."""
+    _chk_cuda(boxes, scores, groups, valid)
+    n = scores.shape[0]
+    m_max = m_max or n
+    dev = scores.device
+    if out is None:
+        out = dict(keep=torch.empty(max_keep, dtype=torch.int32, device=dev), boxes=torch.empty((max_keep, 4), dtype=torch.float32, device=dev),
+                   scores=torch.empty(max_keep, dtype=torch.float32, device=dev), groups=torch.empty(max_keep, dtype=torch.int32, device=dev),
+                   count=torch.empty(1, dtype=torch.int32, device=dev))
+    key = (dev.index, "nms")
+    nb = lib().lwb_det_nms_workspace_bytes(n, m_max)
+    ws = _ws_cache.get(key)
+    if ws is None or ws.numel() < nb:
+        ws = _ws_cache[key] = torch.empty(nb, dtype=torch.uint8, device=dev)
+    _count(4)
+    with _Prof("det", 0.0, "nms"):
+        check(lib().lwb_det_nms(ptr(boxes), ptr(scores), ptr(groups), ptr(valid), n, int(m_max), float(thresh), int(max_keep), ptr(ws),
+                                ptr(out["keep"]), ptr(out["boxes"]), ptr(out["scores"]), ptr(out["groups"]), ptr(out["count"]), stream()),
+              "lwb_det_nms")
+    return out
+
+
+def det_roi_align(feats, boxes, count, out_size, sampling=2, levels=None, y_f32=None, y_hi=None, y_lo=None):
+    """MultiScaleRoIAlign over 4 NHWC fp32 levels [1,h,w,c] -> RoI-major [r_max,out,out,c]."""
+    _chk_cuda(boxes, count, levels, y_f32, y_hi, y_lo, *feats)
+    c = feats[0].shape[-1]
+    fp = (ctypes.c_void_p * 4)(*[f.data_ptr() for f in feats])
+    _count(1)
+    with _Prof("det", 0.0, "roi_align"):
+        check(lib().lwb_det_roi_align(fp, _i32_ptrs([f.shape[1] for f in feats]), _i32_ptrs([f.shape[2] for f in feats]), c,
+                                      ptr(boxes), ptr(count), boxes.shape[0], int(out_size), int(sampling), ptr(levels),
+                                      ptr(y_f32), ptr(y_hi), ptr(y_lo), stream()), "lwb_det_roi_align")
+
+
+def det_box_candidates(pred, nc, proposals, count, clip_hw, score_thresh, min_size, xform_clip, out):
+    _chk_cuda(pred, proposals, count)
+    r_max, ld = pred.shape
+    _count(1)
+    check(lib().lwb_det_box_candidates(ptr(pred), ld, int(nc), ptr(proposals), ptr(count), r_max, float(clip_hw[0]), float(clip_hw[1]),
+                                       float(score_thresh), float(min_size), float(xform_clip), ptr(out["boxes"]), ptr(out["scores"]),
+                                       ptr(out["groups"]), ptr(out["valid"]), stream()), "lwb_det_box_candidates")
+
+
+def det_mask_probs(raw, bias, labels, count, logits=None, probs=None):
+    _chk_cuda(raw, bias, labels, count, logits, probs)
+    d_max, h, w, ld = raw.shape
+    _count(1)
+    check(lib().lwb_det_mask_probs(ptr(raw), ld, ptr(bias), ptr(labels), ptr(count), d_max, h * w, ptr(logits), ptr(probs), stream()),
+          "lwb_det_mask_probs")
+
+
+def det_paste_masks(probs, boxes, count, ratio_hw, hw, masks=None, out_boxes=None):
+    """resize_boxes + paste_masks_in_image: probs [d,m,m], boxes [d,4] -> masks [d,1,h,w] (None: boxes only), boxes [d,4]."""
+    _chk_cuda(probs, boxes, count, masks, out_boxes)
+    d_max, m = probs.shape[0], probs.shape[-1]
+    _count(1)
+    check(lib().lwb_det_paste_masks(ptr(probs), m, ptr(boxes), ptr(count), d_max, float(ratio_hw[0]), float(ratio_hw[1]),
+                                    int(hw[0]), int(hw[1]), ptr(masks), ptr(out_boxes), stream()), "lwb_det_paste_masks")
+
+
+def det_person_mask(boxes, labels, count, masks, thresh, ks, person=1):
+    """-> (pid int32[1], box [4], dilated {0,1} mask [1,1,h,w]) of the largest-area person (the last detection if none)."""
+    _chk_cuda(boxes, labels, count, masks)
+    h, w = masks.shape[-2:]
+    dev = masks.device
+    pid = torch.empty(1, dtype=torch.int32, device=dev)
+    box = torch.empty(4, dtype=torch.float32, device=dev)
+    out = torch.empty((1, 1, h, w), dtype=torch.float32, device=dev)
+    _count(1)
+    check(lib().lwb_det_person_mask(ptr(boxes), ptr(labels), ptr(count), int(person), ptr(masks), h, w, float(thresh), int(ks),
+                                    ptr(pid), ptr(box), ptr(out), stream()), "lwb_det_person_mask")
+    return pid, box, out

@@ -266,6 +266,25 @@ def synthetic_hmr_state(template, seed=4):
     return sd
 
 
+def synthetic_maskrcnn_state(seed=21, person_bias=5.0):
+    """Deterministic weights for the Mask R-CNN detector, with the published COCO checkpoint's (version-1) keys (the
+    44.5 M parameters are regenerated from the seed wherever they are needed).  He-scaled convs and linears, FrozenBN
+    statistics as in fill_state_dict, the last conv of every bottleneck damped (post-add ReLU: 16 unit-gain branches
+    would grow the stream ~30x), the RPN and box predictors damped (objectness and class logits of order 1, as a trained model's: saturated
+    sigmoids would tie), box and anchor deltas small so boxes stay near their anchors / proposals, and the
+    person class's ``cls_score`` bias raised by ``person_bias`` so that several person detections exist."""
+    from .detectors import MaskRCNN, to_v1
+    template = {k: tuple(v.shape) for k, v in MaskRCNN().state_dict().items()}
+    sd = fill_state_dict(template, seed=seed, conv_std='he')
+    for k in sd:
+        if ".conv3." in k and sd[k].dim() == 4:
+            sd[k] = sd[k] * 0.25
+        if k.endswith("bbox_pred.weight") or k.endswith("cls_logits.weight") or k.endswith("cls_score.weight"):
+            sd[k] = sd[k] * 0.1
+    sd["roi_heads.box_predictor.cls_score.bias"][1] += person_bias
+    return to_v1(sd)
+
+
 class QuarterTurnBodyModel(object):
     """A body model whose vertices are EXACT on every device: theta[3] = k selects a rotation of the UV-sphere body by
     k quarter turns about y (a signed permutation of coordinates, no rounding), theta[0:3] = cam.  Used where a CPU-made

@@ -289,6 +289,55 @@ int lwb_smpl_forward(const float* beta, const float* theta, int batch, int num_b
                      float* verts, float* joints, float* Rs, float* J_transformed,
                      const float* cam, float* j2d, void* workspace, lwb_stream_t stream);
 
+/* ---- Mask R-CNN person detector (utils/detectors.py:25-85: torchvision maskrcnn_resnet50_fpn, eval) ------------
+ * The convolutions and fully connected layers run through lwb_conv_plan_*; these are the passes between them.
+ * Every count lives on the device (int32), so a forward pass needs no host synchronisation.  Operands (y_hi, y_lo)
+ * are the conv engine's NHWC fp16 hi / lo pair; either output of a pass may be null when not needed.
+ *   transform     img [3,h,w] in [-1,1] -> (img + 1) / 2, normalised, bilinear to [ho,wo], zero padded: out [3,hp,wp]
+ *   stem_pool     max_pool2d(relu(x * scale + shift), 3, 2, 1): x NCHW fp32 -> operands [n,(h+1)/2,(w+1)/2,c]
+ *   bias_act      y = act(raw[step*(y,x)] + raw2 + bias + res) with res at the same grid or (res_half) nearest 2x from
+ *                 [n,h/2,w/2,c]; raw / raw2 have channel pitch ld_raw on an [h_in,w_in] grid
+ *   d2s_bias_relu ConvTranspose2d(k=2, s=2) from its 1x1 form: raw [n,h,w,4c], column (dy*2+dx)*c + co -> [n,2h,2w,c]
+ *   rpn           per level: top k of the logits (ties to the lower index, sorted), decoded against the anchors,
+ *                 clipped, with sigmoid scores and the small-box filter; heads [gh*gw,16] raw (0..2 logits,
+ *                 3+a*4+k deltas), bias [16]; candidates at offsets[l] of boxes / scores / groups (= level) / valid
+ *   nms           batched NMS over n slots (at most m_max valid): per group greedy, IoU > thresh suppresses; keep
+ *                 = slot indices by descending score (first max_keep, -1 after), gathered boxes / scores / groups
+ *   roi_align     MultiScaleRoIAlign over 4 NHWC levels (scales 1/4..1/32, sampling_ratio, aligned=False) for the
+ *                 first *count of r_max boxes -> RoI-major [r_max,out,out,c] (zeros past *count), levels[r] (nullable)
+ *   box_candidates softmax + per-class decode (10,10,5,5) + clip + filters of pred [r_max, ld] (nc logits, nc*4
+ *                 deltas): slot r*(nc-1)+j-1 for class j
+ *   mask_probs    sigmoid of the label's channel of raw [d_max,hw,ld] + bias
+ *   paste_masks   resize_boxes by (rh, rw) + paste_masks_in_image (padding 1) of probs [d_max,m,m] -> masks [d_max,h,w]
+ *   person_mask   largest-area person (the last detection if none) -> pid, its box, (mask > thresh) dilated by ks */
+int lwb_det_transform(const float* img, int h, int w, int ho, int wo, int hp, int wp, float* out, lwb_stream_t stream);
+int lwb_det_stem_pool(const float* x, int n, int c, int h, int w, const float* scale, const float* shift,
+                      void* y_hi, void* y_lo, lwb_stream_t stream);
+int lwb_det_bias_act(const float* raw, int ld_raw, const float* raw2, const float* bias, const float* res, int res_half,
+                     int step, int h_in, int w_in, int relu, int n, int h, int w, int c,
+                     float* y_f32, void* y_hi, void* y_lo, lwb_stream_t stream);
+int lwb_det_d2s_bias_relu(const float* raw, const float* bias, int n, int h, int w, int c,
+                          float* y_f32, void* y_hi, void* y_lo, lwb_stream_t stream);
+int lwb_det_rpn(int levels, const float* const* heads, const int* gh, const int* gw, const int* stride_h,
+                const int* stride_w, const float* cell_anchors, const int* offsets, const float* bias, int k,
+                float clip_h, float clip_w, float min_size, float xform_clip, int* top_idx, float* boxes,
+                float* scores, int* groups, int* valid, lwb_stream_t stream);
+size_t lwb_det_nms_workspace_bytes(int n, int m_max);
+int lwb_det_nms(const float* boxes, const float* scores, const int* groups, const int* valid, int n, int m_max, float thresh,
+                int max_keep, void* workspace, int* keep, float* out_boxes, float* out_scores, int* out_groups,
+                int* out_count, lwb_stream_t stream);
+int lwb_det_roi_align(const float* const* feats, const int* fh, const int* fw, int c, const float* boxes, const int* count,
+                      int r_max, int out, int sampling, int* levels, float* y_f32, void* y_hi, void* y_lo, lwb_stream_t stream);
+int lwb_det_box_candidates(const float* pred, int ld, int nc, const float* proposals, const int* count, int r_max,
+                           float clip_h, float clip_w, float score_thresh, float min_size, float xform_clip,
+                           float* boxes, float* scores, int* groups, int* valid, lwb_stream_t stream);
+int lwb_det_mask_probs(const float* raw, int ld, const float* bias, const int* labels, const int* count, int d_max, int hw,
+                       float* logits, float* probs, lwb_stream_t stream);
+int lwb_det_paste_masks(const float* probs, int m, const float* boxes, const int* count, int d_max, float rh, float rw,
+                        int h, int w, float* masks, float* out_boxes, lwb_stream_t stream);
+int lwb_det_person_mask(const float* boxes, const int* labels, const int* count, int person, const float* masks, int h, int w,
+                        float thresh, int ks, int* pid, float* box, float* out, lwb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
