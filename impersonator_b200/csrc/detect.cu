@@ -22,10 +22,11 @@ __device__ __forceinline__ float sub(float a, float b) { return __fsub_rn(a, b);
 __device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float dvd(float a, float b) { return __fdiv_rn(a, b); }
 
-// float -> unsigned key with the same order (larger float, larger key)
+// float -> unsigned key with the same order (larger float, larger key).  -0 maps to +0's key: the CPU's stable sort
+// compares them equal and keeps index order between them.
 __device__ __forceinline__ unsigned int order_key(float f)
 {
-    const unsigned int u = __float_as_uint(f);
+    const unsigned int u = __float_as_uint(f == 0.f ? 0.f : f);
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
@@ -731,6 +732,9 @@ extern "C" int lwb_det_person_mask(const float* boxes, const int* labels, const 
 {
     LWB_CHECK_ARG(boxes && labels && count && masks && pid && box && out, "null pointer");
     LWB_CHECK_ARG(h > 0 && w > 0 && ks >= 0, "bad sizes");
+    // utils/util.py morph pads ks // 2 on every side, so an even ks gives an (h+1) x (w+1) mask that the callers'
+    // img * mask cannot broadcast: refuse it here instead of returning a shifted h x w dilation
+    LWB_CHECK_ARG(ks == 0 || ks % 2 == 1, "ks must be 0 or odd");
     k_det_person_mask<<<lwb::ceil_div((long)h * w, 256), 256, 0, (cudaStream_t)stream>>>(boxes, labels, count, person, masks, h, w,
                                                                                         thresh, ks, pid, box, out);
     LWB_LAUNCH_OK();
