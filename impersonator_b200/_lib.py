@@ -67,6 +67,12 @@ SIGNATURES = {
     "lwb_global_avgpool_nhwc": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _i, _vp]),
     "lwb_linear": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "lwb_conv2d_direct_nchw": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "lwb_conv2d_direct_relu_nhwc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "lwb_maxpool_nhwc": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "lwb_ssim_psnr_workspace_bytes": (_sz, [_i, _i, _i]),
+    "lwb_ssim_psnr": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "lwb_lpips_input": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "lwb_lpips_layer": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
     "lwb_det_transform": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "lwb_det_stem_pool": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwb_det_bias_act": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),

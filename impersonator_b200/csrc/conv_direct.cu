@@ -99,7 +99,9 @@ __global__ void k_pack_heads(const float* __restrict__ w_img, const float* __res
 // ------------------------------------------------------------------------------------------
 // generic direct convolution, NCHW fp32 (cold path: once per source image)
 // one thread = one output pixel x 4 output channels; weights are warp-uniform (broadcast loads)
+// NHWC_RELU: relu(out) written NHWC (LPIPS' AlexNet conv1, 11x11 s4, whose output feeds an NHWC pool and a metric tap)
 // ------------------------------------------------------------------------------------------
+template <bool NHWC_RELU>
 __global__ void __launch_bounds__(256) k_conv_direct(const float* __restrict__ x, const float* __restrict__ w,
                                                      const float* __restrict__ bias,
                                                      int cin, int h, int wd, int cout, int kh, int kw,
@@ -132,8 +134,11 @@ __global__ void __launch_bounds__(256) k_conv_direct(const float* __restrict__ x
     }
 #pragma unroll
     for (int j = 0; j < 4; j++)
-        if (co0 + j < cout)
-            out[((size_t)b * cout + co0 + j) * ho * wo + pix] = acc[j] + (bias ? __ldg(bias + co0 + j) : 0.f);
+        if (co0 + j < cout) {
+            const float v = acc[j] + (bias ? __ldg(bias + co0 + j) : 0.f);
+            if (NHWC_RELU) out[((size_t)b * ho * wo + pix) * cout + co0 + j] = fmaxf(v, 0.f);
+            else           out[((size_t)b * cout + co0 + j) * ho * wo + pix] = v;
+        }
 }
 
 }  // namespace
@@ -166,7 +171,21 @@ extern "C" int lwb_conv2d_direct_nchw(const float* x, const float* w, const floa
     const int wo = (wd + 2 * pad - dil * (kw - 1) - 1) / stride + 1;
     LWB_CHECK_ARG(ho > 0 && wo > 0 && n <= 65535, "empty output");
     dim3 grid(lwb::ceil_div((long)ho * wo, 256), lwb::ceil_div(cout, 4), n);
-    k_conv_direct<<<grid, 256, 0, (cudaStream_t)stream>>>(x, w, bias, cin, h, wd, cout, kh, kw, stride, pad, dil, ho, wo, out);
+    k_conv_direct<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, w, bias, cin, h, wd, cout, kh, kw, stride, pad, dil, ho, wo, out);
+    LWB_LAUNCH_OK();
+    return LWB_OK;
+}
+
+extern "C" int lwb_conv2d_direct_relu_nhwc(const float* x, const float* w, const float* bias,
+                                           int n, int cin, int h, int wd, int cout, int kh, int kw,
+                                           int stride, int pad, float* out, lwb_stream_t stream)
+{
+    LWB_CHECK_ARG(x && w && out, "null pointer");
+    LWB_CHECK_ARG(n > 0 && cin > 0 && h > 0 && wd > 0 && cout > 0 && kh > 0 && kw > 0 && stride > 0 && pad >= 0, "bad sizes");
+    const int ho = (h + 2 * pad - kh) / stride + 1, wo = (wd + 2 * pad - kw) / stride + 1;
+    LWB_CHECK_ARG(h + 2 * pad >= kh && wd + 2 * pad >= kw && n <= 65535, "empty output");
+    dim3 grid(lwb::ceil_div((long)ho * wo, 256), lwb::ceil_div(cout, 4), n);
+    k_conv_direct<true><<<grid, 256, 0, (cudaStream_t)stream>>>(x, w, bias, cin, h, wd, cout, kh, kw, stride, pad, 1, ho, wo, out);
     LWB_LAUNCH_OK();
     return LWB_OK;
 }

@@ -30,6 +30,31 @@ __global__ void __launch_bounds__(256) k_maxpool_nchw_to_nhwc(const float* __res
     out[(((size_t)b * ho + oy) * wo + ox) * c + ch] = m;
 }
 
+// F.max_pool2d(x, kernel_size=k, stride=s) with the default ceil_mode=False (torchvision AlexNet's pools): out =
+// floor((in - k) / s) + 1 windows, all inside the input.  NHWC fp32 in -> NHWC fp32 and / or the conv engine's fp16 hi / lo
+// operands.  Consecutive threads walk the channels: coalesced reads and writes.
+__global__ void __launch_bounds__(256) k_maxpool_nhwc(const float* __restrict__ x, int n, int h, int w, int c, int k, int s,
+                                                      int ho, int wo, float* __restrict__ y_f32, __half* __restrict__ y_hi,
+                                                      __half* __restrict__ y_lo)
+{
+    const long total = (long)n * ho * wo * c;
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int ch = (int)(i % c), ox = (int)((i / c) % wo), oy = (int)((i / ((long)c * wo)) % ho), b = (int)(i / ((long)c * wo * ho));
+    const float* p = x + (((size_t)b * h + oy * s) * w + ox * s) * c + ch;
+    float m = -INFINITY;
+    for (int dy = 0; dy < k; dy++)
+        for (int dx = 0; dx < k; dx++)
+            m = fmaxf(m, __ldg(p + ((size_t)dy * w + dx) * c));
+    if (y_f32) y_f32[i] = m;
+    if (y_hi) {
+        __half hi, lo;
+        lwb::split_half(m, hi, lo);
+        y_hi[i] = hi;
+        if (y_lo) y_lo[i] = lo;
+    }
+}
+
 // out[b, ch] = mean over hw of relu?(x[b, p, ch] * scale[ch] + shift[ch])   (post_bn + ReLU + avg_pool2d(7), hmr.py:160-163)
 __global__ void __launch_bounds__(256) k_global_avgpool_nhwc(const float* __restrict__ x, int n, int hw, int c,
                                                              const float* __restrict__ scale, const float* __restrict__ shift,
@@ -80,6 +105,19 @@ extern "C" int lwb_maxpool_nchw_to_nhwc(const float* x, int n, int c, int h, int
     const int ho = lwb::ceil_div(h - k, stride) + 1, wo = lwb::ceil_div(w - k, stride) + 1;
     const long total = (long)n * ho * wo * c;
     k_maxpool_nchw_to_nhwc<<<lwb::ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, n, c, h, w, k, stride, ho, wo, out);
+    LWB_LAUNCH_OK();
+    return LWB_OK;
+}
+
+extern "C" int lwb_maxpool_nhwc(const float* x, int n, int h, int w, int c, int k, int stride, float* y_f32, void* y_hi, void* y_lo,
+                                lwb_stream_t stream)
+{
+    LWB_CHECK_ARG(x && (y_f32 || y_hi), "null pointer");
+    LWB_CHECK_ARG(n > 0 && c > 0 && h >= k && w >= k && k > 0 && stride > 0, "bad sizes");
+    const int ho = (h - k) / stride + 1, wo = (w - k) / stride + 1;
+    const long total = (long)n * ho * wo * c;
+    k_maxpool_nhwc<<<lwb::ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, n, h, w, c, k, stride, ho, wo, y_f32,
+                                                                                (__half*)y_hi, (__half*)y_lo);
     LWB_LAUNCH_OK();
     return LWB_OK;
 }

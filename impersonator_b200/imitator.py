@@ -409,11 +409,21 @@ class Imitator(object):
     @_on_device
     @torch.no_grad()
     def inference(self, tgt_paths, tgt_smpls=None, cam_strategy='smooth', output_dir='', visualizer=None, verbose=True,
-                  as_uint8=False):
+                  as_uint8=False, score_against=None, lpips=None):
         """models/imitator.py:157-189.  Returns per-frame float32 HxWx3 arrays in [-1,1] like the reference; with
         ``as_uint8=True`` (extra) returns the BGR uint8 images the reference writes to disk instead (4x less D2H).
-        With ``output_dir`` the uint8 images come from the GPU and go straight to cv2.imwrite."""
+        With ``output_dir`` the uint8 images come from the GPU and go straight to cv2.imwrite.
+
+        ``score_against`` (extra): ground-truth frames [N,3,H,W] in [-1,1] (numpy or tensor, N = len(tgt_paths)).  Each
+        chunk's frames are scored while still on the device (impersonator_b200.metrics.score_frames: SSIM and PSNR, and
+        LPIPS when an ``lpips`` = metrics.LPIPS is given), and the call returns (outputs, scores) with scores a dict of
+        per-frame float64 numpy arrays."""
         length = len(tgt_paths)
+        if score_against is not None:
+            from . import metrics as _metrics
+            if len(score_against) != length:
+                raise LwbError("score_against holds %d frames for %d targets" % (len(score_against), length))
+            scores = []
         outputs = []
         last_image = [None]
         originals = {}                                           # frame index -> original RGB image (for the gt_ files)
@@ -464,6 +474,9 @@ class Imitator(object):
             want_u8 = bool(as_uint8 or output_dir)
             res = self._chunk_step(smpls, cam_strategy, not as_uint8, want_u8)
             out_hwc, out_u8, flag = res['hwc'], res['u8'], res['flag']
+            if score_against is not None:
+                gt = _metrics._frames(score_against[a:b], self.device)
+                scores.append(_metrics.score_frames(res['preds'], gt, from01=False, lpips=lpips))
             if visualizer is not None:
                 visualizer.vis_named_img('pred_' + cam_strategy, res['preds'])
             ready = torch.cuda.Event()
@@ -481,6 +494,13 @@ class Imitator(object):
             pending.append((a, b, h_f, h_u8, h_flag, done))
             drain(keep=1)
         drain(keep=0)
+
+        def result():
+            if score_against is None:
+                return outputs
+            keys = scores[0].keys() if scores else ("ssim", "psnr")
+            return outputs, {k: torch.cat([s[k].double() for s in scores]).cpu().numpy() if scores else np.zeros(0)
+                             for k in keys}
         self._last_frame_info()
         if last_image[0] is None and length and tgt_paths[-1] and self.tsf_info:
             # driven by given SMPL vectors AND frame files (evaluate.py:62): transfer_params still reads every frame file
@@ -503,7 +523,7 @@ class Imitator(object):
             if os.environ.get("LWB_AUTO_PRECISION", "1") == "0" or getattr(self.generator, '_lwb_precision', None) == "fp16x3" \
                     or os.environ.get("LWB_PRECISION", "fp16f8") != "fp16f8":
                 warnings.warn("lwb_b200: %s (precision mode kept)" % what)
-                return outputs
+                return result()
             warnings.warn("lwb_b200: %s; switching this generator to LWB_PRECISION=fp16x3 and recomputing the sequence" % what)
             self.generator.set_precision("fp16x3")
             self._range_retry = True
@@ -511,10 +531,11 @@ class Imitator(object):
                 enc_in = self.src_info.get('src_inputs')
                 if enc_in is not None:
                     self.src_info['feats'] = self.generator.encode_src(enc_in)
-                return self.inference(tgt_paths, tgt_smpls, cam_strategy, output_dir, visualizer, verbose, as_uint8)
+                return self.inference(tgt_paths, tgt_smpls, cam_strategy, output_dir, visualizer, verbose, as_uint8,
+                                      score_against, lpips)
             finally:
                 self._range_retry = False
-        return outputs
+        return result()
 
     @torch.no_grad()
     def inference_by_smpls(self, tgt_smpls, cam_strategy='smooth', output_dir='', visualizer=None, as_uint8=False):

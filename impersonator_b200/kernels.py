@@ -684,3 +684,82 @@ def det_person_mask(boxes, labels, count, masks, thresh, ks, person=1):
     check(lib().lwb_det_person_mask(ptr(boxes), ptr(labels), ptr(count), int(person), ptr(masks), h, w, float(thresh), int(ks),
                                     ptr(pid), ptr(box), ptr(out), stream()), "lwb_det_person_mask")
     return pid, box, out
+
+
+# ---- paired image-quality metrics (impersonator_b200.metrics) -----------------------------------------------------
+def conv2d_direct_relu_nhwc(x, w, bias=None, stride=1, pad=0, out=None):
+    """relu(conv2d(x, w, bias, stride, pad)): x NCHW fp32 -> NHWC fp32 [n,ho,wo,cout]."""
+    _chk_cuda(x, w, bias, out)
+    n, cin, h, wd = x.shape
+    cout, _, kh, kw = w.shape
+    ho, wo = (h + 2 * pad - kh) // stride + 1, (wd + 2 * pad - kw) // stride + 1
+    if out is None:
+        out = torch.empty((n, ho, wo, cout), dtype=torch.float32, device=x.device)
+    _count(1)
+    check(lib().lwb_conv2d_direct_relu_nhwc(ptr(x), ptr(w), ptr(bias), n, cin, h, wd, cout, kh, kw, stride, pad, ptr(out),
+                                            stream()), "lwb_conv2d_direct_relu_nhwc")
+    return out
+
+
+def maxpool_nhwc(x, k, stride, y_f32=None, y_hi=None, y_lo=None):
+    """F.max_pool2d(x, k, stride) (floor mode) on NHWC fp32 -> y_f32 and / or fp16 hi / lo operands; with no output
+    given, a new fp32 tensor is returned."""
+    _chk_cuda(x, y_f32, y_hi, y_lo)
+    n, h, w, c = x.shape
+    if y_f32 is None and y_hi is None:
+        y_f32 = torch.empty((n, (h - k) // stride + 1, (w - k) // stride + 1, c), dtype=torch.float32, device=x.device)
+    _count(1)
+    check(lib().lwb_maxpool_nhwc(ptr(x), n, h, w, c, k, stride, ptr(y_f32), ptr(y_hi), ptr(y_lo), stream()), "lwb_maxpool_nhwc")
+    return y_f32
+
+
+def _chk_frames(*ts):
+    _chk_cuda(*ts)
+    shape = ts[0].shape
+    for t in ts:
+        if t.dtype != torch.float32 or t.dim() != 4 or t.shape[1] != 3 or t.shape != shape:
+            raise LwbError("frames must be float32 [n,3,h,w] of one shape, got %s / %s" % (tuple(shape), tuple(t.shape)))
+
+
+def ssim_psnr(pred, ref, from01=False, ssim=None, psnr=None):
+    """Per-frame SSIM and PSNR (lwb_ssim_psnr) of [n,3,h,w] fp32 frames in [-1,1] ([0,1] with from01) -> fp64 [n], [n]."""
+    _chk_frames(pred, ref)
+    n, _, h, w = pred.shape
+    dev = pred.device
+    if ssim is None:
+        ssim = torch.empty(n, dtype=torch.float64, device=dev)
+        psnr = torch.empty(n, dtype=torch.float64, device=dev)
+    key = (dev.index, "ssim")
+    nb = lib().lwb_ssim_psnr_workspace_bytes(n, h, w)
+    ws = _ws_cache.get(key)
+    if ws is None or ws.numel() < nb:
+        ws = _ws_cache[key] = torch.empty(nb, dtype=torch.uint8, device=dev)
+    _count(2)
+    with _Prof("metrics", 0.0, "ssim_psnr"):
+        check(lib().lwb_ssim_psnr(ptr(pred), ptr(ref), n, h, w, 1 if from01 else 0, ptr(ws), ptr(ssim), ptr(psnr), stream()),
+              "lwb_ssim_psnr")
+    return ssim, psnr
+
+
+def lpips_input(pred, ref, from01=False, out=None):
+    """PNetLin's scaling layer of pred and ref as one batch [2n,3,h,w] (pred first)."""
+    _chk_frames(pred, ref)
+    n, _, h, w = pred.shape
+    if out is None:
+        out = torch.empty((2 * n, 3, h, w), dtype=torch.float32, device=pred.device)
+    _chk_cuda(out)
+    _count(1)
+    check(lib().lwb_lpips_input(ptr(pred), ptr(ref), n, h, w, 1 if from01 else 0, ptr(out), stream()), "lwb_lpips_input")
+    return out
+
+
+def lpips_layer(feat, lin, layer, layers, score):
+    """One LPIPS tap of feat NHWC [2n,h,w,c] into layers [n, L] (column ``layer``) and score [n] (= for layer 0, += after)."""
+    _chk_cuda(feat, lin, layers, score)
+    n2, h, w, c = feat.shape
+    if lin.numel() != c or layers.dim() != 2 or layers.shape[0] != n2 // 2 or score.numel() != n2 // 2:
+        raise LwbError("lpips_layer: %d channels, %d lin weights, layers %s, score %s" % (c, lin.numel(), tuple(layers.shape),
+                                                                                           tuple(score.shape)))
+    _count(1)
+    check(lib().lwb_lpips_layer(ptr(feat), n2 // 2, h * w, c, ptr(lin), int(layer), layers.shape[1], ptr(layers), ptr(score),
+                                stream()), "lwb_lpips_layer")

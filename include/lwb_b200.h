@@ -232,6 +232,10 @@ int lwb_frames_out(const float* frames, int n, int h, int w, float* hwc, uint8_t
 int lwb_conv2d_direct_nchw(const float* x, const float* w, const float* bias,
                            int n, int cin, int h, int wd, int cout, int kh, int kw,
                            int stride, int pad, int dil, float* out, lwb_stream_t stream);
+/* The same convolution (dilation 1) with relu(out) written NHWC [n,ho,wo,cout]: LPIPS' AlexNet conv1 (11x11 s4 p2). */
+int lwb_conv2d_direct_relu_nhwc(const float* x, const float* w, const float* bias,
+                                int n, int cin, int h, int wd, int cout, int kh, int kw,
+                                int stride, int pad, float* out, lwb_stream_t stream);
 
 /* Gated-conv epilogue of the inpaintor (networks/inpaintor.py:37-47): ab [n,2c,h,w] = conv2d(x) and
  * mask_conv2d(x) stacked on channels; out [n,c,h,w] = (act(a) * sigmoid(b)) * scale[c] + shift[c]
@@ -265,6 +269,10 @@ int lwb_self_attention_nhwc(const float* qkv, int ld, const float* bias, int n, 
  *     out[b*ld_out + ch]
  *   nn.Linear (+ReLU) of the theta regressor (hmr.py:223-252): out[b*ld_out + j] (+)= relu?(x[b*ld_x + :k] . w[j,:k] + bias[j]) */
 int lwb_maxpool_nchw_to_nhwc(const float* x, int n, int c, int h, int w, int k, int stride, float* out, lwb_stream_t stream);
+/* F.max_pool2d(x, k, stride) in floor mode (ceil_mode=False, AlexNet's pools), x NHWC fp32 [n,h,w,c] -> [n,ho,wo,c],
+ * ho = (h-k)/stride+1: fp32 (y_f32) and / or the conv engine's fp16 hi / lo operands (y_lo nullable); either may be null. */
+int lwb_maxpool_nhwc(const float* x, int n, int h, int w, int c, int k, int stride, float* y_f32, void* y_hi, void* y_lo,
+                     lwb_stream_t stream);
 int lwb_global_avgpool_nhwc(const float* x, int n, int hw, int c, const float* scale, const float* shift, int relu,
                             float* out, int ld_out, lwb_stream_t stream);
 int lwb_linear(const float* x, int ld_x, const float* w, const float* bias, int n, int k, int m, int relu, int accumulate,
@@ -337,6 +345,27 @@ int lwb_det_paste_masks(const float* probs, int m, const float* boxes, const int
                         int h, int w, float* masks, float* out_boxes, lwb_stream_t stream);
 int lwb_det_person_mask(const float* boxes, const int* labels, const int* count, int person, const float* masks, int h, int w,
                         float thresh, int ks, int* pid, float* box, float* out, lwb_stream_t stream);
+
+/* ---- Paired image-quality metrics (his_evaluators/metrics/metrics.py:450-631) --------------------------------------
+ * pred / ref: [n,3,h,w] fp32 NCHW in [-1,1], or in [0,1] with from01 = 1 (mapped by x * 2 - 1 in fp32, as the metrics'
+ * preprocess does).
+ *   ssim_psnr     per frame: skimage 0.16.2 structural_similarity(pred, ref, multichannel=True) on the HWC image (7x7
+ *                 uniform window, sample covariance, K1 0.01, K2 0.03, data_range 2, map cropped by 3, mean per channel
+ *                 then over channels) and peak_signal_noise_ratio(image_true=ref, image_test=pred) (data_range 1 when
+ *                 min(ref) >= 0, else 2; +inf for identical frames), both fp64 [n].  h, w >= 7.  workspace:
+ *                 lwb_ssim_psnr_workspace_bytes(n, h, w) bytes.  Fixed-order reductions: results repeat bit for bit.
+ *   lpips_input   PNetLin's scaling layer (x - shift) / scale of pred and ref stacked as one batch: out [2n,3,h,w]
+ *                 (pred first), the input of the AlexNet features (conv1 via lwb_conv2d_direct_relu_nhwc, the pools via
+ *                 lwb_maxpool_nhwc, conv2..5 via lwb_conv_plan_* + lwb_det_bias_act).
+ *   lpips_layer   one tap: feat NHWC [2n,hw,c] (pred features = image i, ref = image n+i); per frame the spatial mean of
+ *                 sum_c lin[c] * (f0/(|f0|+1e-10) - f1/(|f1|+1e-10))^2 -> layers_out[i*num_layers + layer]; score[i] =
+ *                 that value for layer 0, score[i] + it after (run the taps in order on one stream). */
+size_t lwb_ssim_psnr_workspace_bytes(int n, int h, int w);
+int lwb_ssim_psnr(const float* pred, const float* ref, int n, int h, int w, int from01, void* workspace,
+                  double* ssim_out, double* psnr_out, lwb_stream_t stream);
+int lwb_lpips_input(const float* pred, const float* ref, int n, int h, int w, int from01, float* out, lwb_stream_t stream);
+int lwb_lpips_layer(const float* feat, int n, int hw, int c, const float* lin, int layer, int num_layers,
+                    float* layers_out, float* score, lwb_stream_t stream);
 
 #ifdef __cplusplus
 }
