@@ -73,6 +73,9 @@ SIGNATURES = {
     "lwb_ssim_psnr": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "lwb_lpips_input": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "lwb_lpips_layer": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
+    "lwb_inception_input": (_i, [_vp, _i, _i, _i, _vp, _vp]),
+    "lwb_bn_act_segment": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _vp]),
+    "lwb_maxpool_nhwc_slice": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
     "lwb_det_transform": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "lwb_det_stem_pool": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "lwb_det_bias_act": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),

@@ -32,26 +32,31 @@ __global__ void __launch_bounds__(256) k_maxpool_nchw_to_nhwc(const float* __res
 
 // F.max_pool2d(x, kernel_size=k, stride=s) with the default ceil_mode=False (torchvision AlexNet's pools): out =
 // floor((in - k) / s) + 1 windows, all inside the input.  NHWC fp32 in -> NHWC fp32 and / or the conv engine's fp16 hi / lo
-// operands.  Consecutive threads walk the channels: coalesced reads and writes.
-__global__ void __launch_bounds__(256) k_maxpool_nhwc(const float* __restrict__ x, int n, int h, int w, int c, int k, int s,
-                                                      int ho, int wo, float* __restrict__ y_f32, __half* __restrict__ y_hi,
-                                                      __half* __restrict__ y_lo)
+// operands.  Consecutive threads walk the channels: coalesced reads and writes.  Channels [0, c) of an input with
+// channel pitch ld_x land in channels [off_y, off_y + c) of outputs with pitch ld_y (InceptionV3's Mixed_6a / 7a pool
+// branches write their slice of the block's concat buffer this way).
+__global__ void __launch_bounds__(256) k_maxpool_nhwc(const float* __restrict__ x, int n, int h, int w, int c, int ld_x, int k,
+                                                      int s, int ho, int wo, float* __restrict__ y_f32, __half* __restrict__ y_hi,
+                                                      __half* __restrict__ y_lo, int ld_y, int off_y)
 {
     const long total = (long)n * ho * wo * c;
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const int ch = (int)(i % c), ox = (int)((i / c) % wo), oy = (int)((i / ((long)c * wo)) % ho), b = (int)(i / ((long)c * wo * ho));
-    const float* p = x + (((size_t)b * h + oy * s) * w + ox * s) * c + ch;
+    const int ch = (int)(i % c);
+    const long pix = i / c;
+    const int ox = (int)(pix % wo), oy = (int)((pix / wo) % ho), b = (int)(pix / ((long)wo * ho));
+    const float* p = x + (((size_t)b * h + oy * s) * w + ox * s) * ld_x + ch;
     float m = -INFINITY;
     for (int dy = 0; dy < k; dy++)
         for (int dx = 0; dx < k; dx++)
-            m = fmaxf(m, __ldg(p + ((size_t)dy * w + dx) * c));
-    if (y_f32) y_f32[i] = m;
+            m = fmaxf(m, __ldg(p + ((size_t)dy * w + dx) * ld_x));
+    const size_t o = (size_t)pix * ld_y + off_y + ch;
+    if (y_f32) y_f32[o] = m;
     if (y_hi) {
         __half hi, lo;
         lwb::split_half(m, hi, lo);
-        y_hi[i] = hi;
-        if (y_lo) y_lo[i] = lo;
+        y_hi[o] = hi;
+        if (y_lo) y_lo[o] = lo;
     }
 }
 
@@ -116,8 +121,22 @@ extern "C" int lwb_maxpool_nhwc(const float* x, int n, int h, int w, int c, int 
     LWB_CHECK_ARG(n > 0 && c > 0 && h >= k && w >= k && k > 0 && stride > 0, "bad sizes");
     const int ho = (h - k) / stride + 1, wo = (w - k) / stride + 1;
     const long total = (long)n * ho * wo * c;
-    k_maxpool_nhwc<<<lwb::ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, n, h, w, c, k, stride, ho, wo, y_f32,
-                                                                                (__half*)y_hi, (__half*)y_lo);
+    k_maxpool_nhwc<<<lwb::ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, n, h, w, c, c, k, stride, ho, wo, y_f32,
+                                                                                (__half*)y_hi, (__half*)y_lo, c, 0);
+    LWB_LAUNCH_OK();
+    return LWB_OK;
+}
+
+extern "C" int lwb_maxpool_nhwc_slice(const float* x, int n, int h, int w, int c, int ld_x, int k, int stride, float* y_f32,
+                                      void* y_hi, void* y_lo, int ld_y, int off_y, lwb_stream_t stream)
+{
+    LWB_CHECK_ARG(x && (y_f32 || y_hi), "null pointer");
+    LWB_CHECK_ARG(n > 0 && c > 0 && h >= k && w >= k && k > 0 && stride > 0, "bad sizes");
+    LWB_CHECK_ARG(ld_x >= c && off_y >= 0 && off_y + c <= ld_y, "channel slice outside the pitch");
+    const int ho = (h - k) / stride + 1, wo = (w - k) / stride + 1;
+    const long total = (long)n * ho * wo * c;
+    k_maxpool_nhwc<<<lwb::ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, n, h, w, c, ld_x, k, stride, ho, wo, y_f32,
+                                                                                (__half*)y_hi, (__half*)y_lo, ld_y, off_y);
     LWB_LAUNCH_OK();
     return LWB_OK;
 }

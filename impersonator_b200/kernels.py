@@ -763,3 +763,49 @@ def lpips_layer(feat, lin, layer, layers, score):
     _count(1)
     check(lib().lwb_lpips_layer(ptr(feat), n2 // 2, h * w, c, ptr(lin), int(layer), layers.shape[1], ptr(layers), ptr(score),
                                 stream()), "lwb_lpips_layer")
+
+
+# ---- unpaired image-quality metrics: InceptionV3 features (impersonator_b200.metrics) ------------------------------
+def inception_input(x, out=None):
+    """[n,3,h,w] fp32 frames in [0,1] -> x * 2 - 1 bilinearly resized to [n,3,299,299] (align_corners=False)."""
+    _chk_frames(x)
+    n, _, h, w = x.shape
+    if out is None:
+        out = torch.empty((n, 3, 299, 299), dtype=torch.float32, device=x.device)
+    _chk_cuda(out)
+    if tuple(out.shape) != (n, 3, 299, 299):
+        raise LwbError("inception_input: out must be [%d,3,299,299], got %s" % (n, tuple(out.shape)))
+    _count(1)
+    check(lib().lwb_inception_input(ptr(x), n, h, w, ptr(out), stream()), "lwb_inception_input")
+    return out
+
+
+def bn_act_segment(raw, c0, c, scale=None, shift=None, relu=True, box=False, c_out=None, y_f32=None, y_hi=None, y_lo=None,
+                   off_y=0):
+    """relu?(r * scale + shift) of channels [c0, c0+c) of raw NHWC fp32 [n,h,w,ld] (r = their 3x3 box mean / 9 with
+    ``box``) -> channels [off_y, off_y + c_out) of y_f32 and / or fp16 y_hi / y_lo (one pitch, channels >= c zero)."""
+    _chk_cuda(raw, scale, shift, y_f32, y_hi, y_lo)
+    n, h, w, ld = raw.shape
+    c_out = c_out or c
+    ys = [t for t in (y_f32, y_hi, y_lo) if t is not None]
+    if not ys or any(t.shape[:3] != raw.shape[:3] or t.shape[3] != ys[0].shape[3] for t in ys):
+        raise LwbError("bn_act_segment: outputs must be [%d,%d,%d,pitch] of one pitch" % (n, h, w))
+    if scale is not None and (scale.numel() != c or shift.numel() != c):
+        raise LwbError("bn_act_segment: scale / shift must hold %d values" % c)
+    _count(1)
+    check(lib().lwb_bn_act_segment(ptr(raw), n, h, w, ld, int(c0), int(c), int(c_out), 1 if box else 0, ptr(scale), ptr(shift),
+                                   1 if relu else 0, ptr(y_f32), ptr(y_hi), ptr(y_lo), ys[0].shape[3], int(off_y), stream()),
+          "lwb_bn_act_segment")
+
+
+def maxpool_nhwc_slice(x, c, k, stride, y_f32=None, y_hi=None, y_lo=None, off_y=0):
+    """F.max_pool2d(x[..., :c], k, stride) (floor mode) of NHWC fp32 x -> channels [off_y, off_y + c) of the outputs."""
+    _chk_cuda(x, y_f32, y_hi, y_lo)
+    n, h, w, ld_x = x.shape
+    ys = [t for t in (y_f32, y_hi, y_lo) if t is not None]
+    ho, wo = (h - k) // stride + 1, (w - k) // stride + 1
+    if not ys or any(tuple(t.shape[:3]) != (n, ho, wo) or t.shape[3] != ys[0].shape[3] for t in ys):
+        raise LwbError("maxpool_nhwc_slice: outputs must be [%d,%d,%d,pitch] of one pitch" % (n, ho, wo))
+    _count(1)
+    check(lib().lwb_maxpool_nhwc_slice(ptr(x), n, h, w, int(c), ld_x, k, stride, ptr(y_f32), ptr(y_hi), ptr(y_lo),
+                                       ys[0].shape[3], int(off_y), stream()), "lwb_maxpool_nhwc_slice")

@@ -367,6 +367,25 @@ int lwb_lpips_input(const float* pred, const float* ref, int n, int h, int w, in
 int lwb_lpips_layer(const float* feat, int n, int hw, int c, const float* lin, int layer, int num_layers,
                     float* layers_out, float* score, lwb_stream_t stream);
 
+/* ---- Unpaired image-quality metrics: InceptionV3 features (his_evaluators/metrics/metrics.py:16-158, 634-781) -------
+ *   inception_input   x [n,3,h,w] fp32 in [0,1] -> out [n,3,299,299]: x * 2 - 1, then F.interpolate(size=(299, 299),
+ *                     mode='bilinear', align_corners=False) in fp32 (the metric classes' preprocess).  The stem is
+ *                     lwb_conv2d_direct_relu_nhwc with BN folded into its weights and bias, the other 93 convolutions
+ *                     the conv engine (lwb_conv_plan_*).
+ *   bn_act_segment    channels [c0, c0+c) of a raw NHWC fp32 conv output [n,h,w,ld_raw] -> v = relu?(r * scale + shift),
+ *                     r = the raw value, or with box = 1 its 3x3 zero-padded box sum / 9 (avg_pool2d(3, 1, 1) commutes
+ *                     with the bias-free 1x1 conv of an Inception pool branch); scale / shift [c] or both null
+ *                     (identity).  Written to channels [off_y, off_y+c_out) of fp32 y_f32 and / or fp16 hi / lo operands
+ *                     y_hi, y_lo (nullable) of pitch ld_y, channels c..c_out-1 zero.
+ *   maxpool_nhwc_slice  lwb_maxpool_nhwc of channels [0, c) of x (pitch ld_x) into channels [off_y, off_y+c) of outputs
+ *                     with pitch ld_y (the Mixed_6a / 7a pool branches into their concat buffer). */
+int lwb_inception_input(const float* x, int n, int h, int w, float* out, lwb_stream_t stream);
+int lwb_bn_act_segment(const float* raw, int n, int h, int w, int ld_raw, int c0, int c, int c_out, int box,
+                       const float* scale, const float* shift, int relu, float* y_f32, void* y_hi, void* y_lo,
+                       int ld_y, int off_y, lwb_stream_t stream);
+int lwb_maxpool_nhwc_slice(const float* x, int n, int h, int w, int c, int ld_x, int k, int stride, float* y_f32,
+                           void* y_hi, void* y_lo, int ld_y, int off_y, lwb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
