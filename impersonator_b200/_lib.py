@@ -48,6 +48,8 @@ SIGNATURES = {
                                   ctypes.POINTER(_vp)]),
     "lwb_conv_plan_run": (_i, [_vp, _vp]),
     "lwb_conv_plan_num_launches": (_i, [_vp]),
+    "lwb_conv_kernel_resources": (_i, [_i, _i, _vp]),
+    "lwb_glue_kernel_resources": (_i, [_i, _i, _vp]),
     "lwb_conv_plan_destroy": (None, [_vp]),
     "lwb_conv2d_nhwc": (_i, [ctypes.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lwb_instance_stats_nhwc": (_i, [_vp, _i, _i, _i, _i, _vp, _vp]),

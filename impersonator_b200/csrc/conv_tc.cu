@@ -11,8 +11,9 @@
 //           (out-of-bounds rows/cols are zero-filled by the TMA unit = the conv padding),
 //   W     = weights repacked once to [tap][Cout][Cin] fp16 (K-major rows of 128 bytes).
 // Both operands land in shared memory in the canonical K-major SWIZZLE_128B layout.  A CTA is one
-// TMA producer warp and two consumer warpgroups; each consumer warpgroup owns 64 rows of the tile
-// and issues, per tap and K = 64 chunk, 4 x wgmma (M64 x N_TILE x K16) into register accumulators.
+// producer warpgroup (one warp issues the TMA loads, see Regs) and two consumer warpgroups; each consumer
+// warpgroup owns 64 rows of the tile and issues, per tap and K = 64 chunk, 4 x wgmma (M64 x N_TILE x K16)
+// into register accumulators.
 //
 // Y-halo tap groups: one image row of the tile (8 px x 128 B) is exactly one 1024-byte swizzle atom, so
 // taps that read the same input view at the same dx with consecutive dy share ONE activation box of
@@ -65,7 +66,7 @@ constexpr int MAX_GROUP = 8;                     // taps per y-halo group: A box
 constexpr int RING_BYTES = 200 * 1024;           // A ring + B ring
 constexpr int MAX_STAGES = 8;                    // entries per ring
 constexpr int NUM_CONSUMERS = 256;               // warps 0..7: two consumer warpgroups
-constexpr int NUM_THREADS = NUM_CONSUMERS + 32;  // warp 8: TMA producer
+constexpr int NUM_THREADS = NUM_CONSUMERS + 128; // warps 8..11: producer warpgroup (warp 8 issues the TMA loads)
 constexpr int MAX_N_TILE = 128;                  // 64 fp32 accumulator registers per consumer thread
 static_assert(2 * 2 * (TILE_H + MAX_GROUP - 1) * ROW_BYTES + 2 * 2 * MAX_N_TILE * 128 <= RING_BYTES,
               "every plan needs two A and two B entries in the ring");
@@ -213,7 +214,7 @@ template <> __device__ __forceinline__ void wgmma_e4m3<128>(float* d, uint64_t d
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// Persistent tile schedule shared by the producer warp and the consumer warpgroups: tile = blockIdx.x + k * gridDim.x,
+// Persistent tile schedule shared by the producer and the consumer warpgroups: tile = blockIdx.x + k * gridDim.x,
 // N tile = tile / m_tiles (consecutive tiles share the weight tile and run through the images in order).
 struct TileCoord {
     int n_idx, img, y0, x0;
@@ -375,6 +376,22 @@ __device__ __forceinline__ void epilogue_swapped(const ConvParams& P, float* acc
 // product + one e4m3 wgmma on the lo pair blocks (A entries then hold [A_hi | A_lo8], B entries [B_hi | B_lo8]).
 enum { MODE_FP16 = 0, MODE_FP16X3 = 1, MODE_F8 = 2 };
 
+// Register budget per thread (setmaxnreg).  Registers are allocated per SM sub-partition (16 K each), and warp w of a CTA
+// lands on sub-partition w % 4.  A CTA of two consumer warpgroups and one producer warp at the consumers' 161 registers
+// (fp16f8) put three 168-register warps on sub-partition 0 and left 256 registers there, so no 256-thread block of any
+// other kernel (k_norm_act of the other sub-batch stream) could become resident beside a conv CTA.  With a producer
+// warpgroup the CTA launches at LAUNCH registers per thread (three warps per sub-partition), the producer warpgroup gives
+// all but PRODUCER back and the consumers take CONSUMER: 2 CONSUMER + PRODUCER = 3 LAUNCH, and every sub-partition keeps
+// 16 K - 3 x 32 LAUNCH registers for other kernels (4 K, one 64-register warp pair, for the fp16f8 instances).
+// CONSUMER is at least what ptxas needs for the consumer path of the instance (no spills, see -Xptxas -v).
+template <int N_TILE, int MODE>
+struct Regs {
+    static constexpr int CONSUMER = N_TILE >= 64 ? (MODE == MODE_F8 ? 168 : 120) : N_TILE == 32 ? 80 : 64;
+    static constexpr int LAUNCH = ((2 * CONSUMER + 40 + 2) / 3 + 7) / 8 * 8;
+    static constexpr int PRODUCER = 3 * LAUNCH - 2 * CONSUMER;
+    static_assert(PRODUCER >= 40 && PRODUCER % 8 == 0 && CONSUMER % 8 == 0, "setmaxnreg takes multiples of 8");
+};
+
 // One fp16 wgmma step of the tile: activation rows x weight rows, or (SWAP) weight rows x activation rows on 128 pixels.
 template <int N_TILE, bool SWAP>
 __device__ __forceinline__ void mma_f16(float* d, uint64_t act, uint64_t w) {
@@ -388,7 +405,8 @@ __device__ __forceinline__ void mma_e4m3(float* d, uint64_t act, uint64_t w) {
 }
 
 template <int N_TILE, int MODE>
-__global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constant__ ConvParams P)
+__global__ void __launch_bounds__(NUM_THREADS, 1) __maxnreg__((Regs<N_TILE, MODE>::LAUNCH))
+k_conv_wg(const __grid_constant__ ConvParams P)
 {
     // N tile 64 always runs the swapped orientation (256-pixel tiles, see the top of the file); plan creation sized its
     // tiles and boxes with tile_rows(n_tile) to match.
@@ -428,8 +446,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
     const int m_tiles = P.n_img * P.tiles_y * P.tiles_x;
     const int total = m_tiles * P.n_tiles_n;
 
-    if (warp == NUM_CONSUMERS / 32) {
-        // ================================ TMA producer (whole warp, one elected lane issues) ==========
+    if (warp >= NUM_CONSUMERS / 32) {
+        // ================================ TMA producer (warp 8; one elected lane issues) ==============
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(Regs<N_TILE, MODE>::PRODUCER));
+        if (warp != NUM_CONSUMERS / 32) return;
         if (elect_one()) {
             asm volatile("prefetch.tensormap [%0];" :: "l"(&P.a_hi[0]) : "memory");
             asm volatile("prefetch.tensormap [%0];" :: "l"(&P.w_hi) : "memory");
@@ -473,8 +493,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_wg(const __grid_constan
                 }
             }
         }
-    } else if (warp < NUM_CONSUMERS / 32) {
+    } else {
         // ================================ consumers (2 warpgroups, half of the tile rows each) ========
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(Regs<N_TILE, MODE>::CONSUMER));
         const uint32_t smem_base = smem_u32(smem);
         const uint32_t b_base = smem_u32(b_ring);
         const uint32_t a_row0 = (uint32_t)(warp >> 2) * (TH / 2) * ROW_BYTES;   // tile rows (TH/2) g .. (TH/2)(g + 1) - 1
@@ -914,4 +935,42 @@ extern "C" int lwb_conv2d_nhwc(const lwb_conv_desc* d,
     rc = lwb_conv_plan_run(plan, stream);
     lwb_conv_plan_destroy(plan);
     return rc;
+}
+
+// Resources of one k_conv_wg instance as launched: [registers per thread at launch, static smem, dynamic smem, local
+// bytes per thread, threads per CTA, CTAs per SM alone (occupancy API), consumer registers after setmaxnreg].
+template <int N_TILE, int MODE>
+static int conv_resources(int* out)
+{
+    using C = Cfg<N_TILE, MODE != MODE_FP16>;
+    cudaFuncAttributes a;
+    LWB_CUDA_OK(cudaFuncSetAttribute(k_conv_wg<N_TILE, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    LWB_CUDA_OK(cudaFuncGetAttributes(&a, k_conv_wg<N_TILE, MODE>));
+    int blocks = 0;
+    LWB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, k_conv_wg<N_TILE, MODE>, NUM_THREADS, C::SMEM_BYTES));
+    out[0] = a.numRegs; out[1] = (int)a.sharedSizeBytes; out[2] = C::SMEM_BYTES; out[3] = (int)a.localSizeBytes;
+    out[4] = NUM_THREADS; out[5] = blocks; out[6] = Regs<N_TILE, MODE>::CONSUMER;
+    return LWB_OK;
+}
+
+extern "C" int lwb_conv_kernel_resources(int n_tile, int mode, int* out)
+{
+    LWB_CHECK_ARG(out, "null pointer");
+    LWB_CHECK_ARG(mode >= 0 && mode <= 2, "mode must be 0, 1 or 2");
+    switch (n_tile * 4 + mode) {
+        case 16 * 4 + 0:  return conv_resources<16, 0>(out);
+        case 16 * 4 + 1:  return conv_resources<16, 1>(out);
+        case 16 * 4 + 2:  return conv_resources<16, 2>(out);
+        case 32 * 4 + 0:  return conv_resources<32, 0>(out);
+        case 32 * 4 + 1:  return conv_resources<32, 1>(out);
+        case 32 * 4 + 2:  return conv_resources<32, 2>(out);
+        case 64 * 4 + 0:  return conv_resources<64, 0>(out);
+        case 64 * 4 + 1:  return conv_resources<64, 1>(out);
+        case 64 * 4 + 2:  return conv_resources<64, 2>(out);
+        case 128 * 4 + 0: return conv_resources<128, 0>(out);
+        case 128 * 4 + 1: return conv_resources<128, 1>(out);
+        case 128 * 4 + 2: return conv_resources<128, 2>(out);
+    }
+    lwb::set_error("conv_tc: unsupported N tile %d", n_tile);
+    return LWB_E_UNSUPPORTED;
 }

@@ -223,11 +223,14 @@ struct NormActParams {
 // that four 16B loads per operand are in flight before any math.  The bilinear taps of a pixel are
 // computed once (by one thread) and shared through smem instead of once per channel octet.
 struct TapRec { int o00, m; float w00, w01, w10, w11; };
+constexpr int kNormRounds = 2;                           // pixel rounds per thread
 
+// WARP: the launch's dynamic shared memory holds the ppb * R tap records of the block (768 bytes at 128 channels), so
+// that the block fits beside a resident conv CTA (about 17 KB of shared memory left, conv_tc.cu).
 template <bool WARP, bool EXT>
 __global__ void __launch_bounds__(256, 4) k_norm_act(NormActParams P)
 {
-    constexpr int R = 2;                                 // pixel rounds per thread
+    constexpr int R = kNormRounds;
     lwb::pdl_wait();                                     // raw / scale-shift / residual come from the kernels before
     lwb::pdl_trigger();                                  // the next conv may set up while this grid drains
     const int groups = P.c >> 3;
@@ -236,9 +239,9 @@ __global__ void __launch_bounds__(256, 4) k_norm_act(NormActParams P)
     const long npix = (long)P.n * P.h * P.w;
     const int hw = P.h * P.w;
     const long pix0 = (long)blockIdx.x * (ppb * R);
-    __shared__ TapRec s_tap[512];                      // ppb * R <= 512 (c = 8)
+    extern __shared__ TapRec s_tap[];                    // WARP: ppb * R records
     if (WARP) {
-        for (int i = threadIdx.x; i < ppb * R; i += 256) {       // ppb * R = 512 when c == 8
+        for (int i = threadIdx.x; i < ppb * R; i += 256) {
             const long pg = pix0 + i;
             TapRec t = {0, 0, 0.f, 0.f, 0.f, 0.f};
             if (pg < npix) {
@@ -272,7 +275,7 @@ __global__ void __launch_bounds__(256, 4) k_norm_act(NormActParams P)
         }
     }
     float res[R][8];
-    if (P.residual) {
+    if (P.residual && !WARP) {                           // WARP loads it per round: the warp taps need the registers
 #pragma unroll
         for (int r = 0; r < R; r++) {
             size_t roff = off[r];
@@ -303,6 +306,13 @@ __global__ void __launch_bounds__(256, 4) k_norm_act(NormActParams P)
             for (int k = 0; k < 8; k++) v[r][k] = fmaxf(v[r][k], 0.f);
         }
         if (P.residual) {
+            if (WARP) {
+                if (ok[r]) lwb::ldg_f32x8(P.residual + off[r], res[r]);
+                else {
+#pragma unroll
+                    for (int k = 0; k < 8; k++) res[r][k] = 0.f;
+                }
+            }
 #pragma unroll
             for (int k = 0; k < 8; k++) v[r][k] += res[r][k];
         }
@@ -590,8 +600,10 @@ extern "C" int lwb_norm_act_nhwc(const float* raw, const double* stats, const fl
     P.y_f32 = y_f32; P.y_hi = (__half*)y_hi; P.y_lo = (__half*)y_lo; P.lo_format = lo_format;
     const int groups = c / 8;
     LWB_CHECK_ARG(groups <= 256 && 256 % groups == 0, "channels / 8 must divide 256");
-    const long blocks = lwb::ceil_div((long)n * h * w, (256 / groups) * 2);
-    if (warp_src) LWB_CUDA_OK(lwb::launch_pdl(k_norm_act<true, false>, dim3((unsigned)blocks), dim3(256), 0, st, P));
+    const int px_per_block = (256 / groups) * kNormRounds;
+    const long blocks = lwb::ceil_div((long)n * h * w, px_per_block);
+    if (warp_src) LWB_CUDA_OK(lwb::launch_pdl(k_norm_act<true, false>, dim3((unsigned)blocks), dim3(256),
+                                              px_per_block * sizeof(TapRec), st, P));
     else if (ext) LWB_CUDA_OK(lwb::launch_pdl(k_norm_act<false, true>, dim3((unsigned)blocks), dim3(256), 0, st, P));
     else          LWB_CUDA_OK(lwb::launch_pdl(k_norm_act<false, false>, dim3((unsigned)blocks), dim3(256), 0, st, P));
     return LWB_OK;
@@ -619,4 +631,34 @@ extern "C" int lwb_frames_out(const float* frames, int n, int h, int w, float* h
     k_frames_out<<<lwb::ceil_div((long)n * h * w, 256), 256, 0, (cudaStream_t)stream>>>(frames, n, h * w, hwc, u8_bgr);
     LWB_LAUNCH_OK();
     return LWB_OK;
+}
+
+// Resources of the HBM-bound kernels that run beside the convolutions of the other sub-batch stream: which = 0
+// k_norm_act (plain), 1 k_norm_act<WARP> at c channels, 2 k_norm_act<EXT>, 3 k_heads, 4 k_nchw_to_nhwc_split.
+// out: [registers per thread, static smem, dynamic smem, local bytes per thread, threads per block, blocks per SM alone].
+template <typename F>
+static int glue_resources(F* fn, int threads, int dyn_smem, int* out)
+{
+    cudaFuncAttributes a;
+    LWB_CUDA_OK(cudaFuncGetAttributes(&a, fn));
+    int blocks = 0;
+    LWB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, fn, threads, dyn_smem));
+    out[0] = a.numRegs; out[1] = (int)a.sharedSizeBytes; out[2] = dyn_smem; out[3] = (int)a.localSizeBytes;
+    out[4] = threads; out[5] = blocks;
+    return LWB_OK;
+}
+
+extern "C" int lwb_glue_kernel_resources(int which, int c, int* out)
+{
+    LWB_CHECK_ARG(out, "null pointer");
+    LWB_CHECK_ARG(which != 1 || (c >= 16 && c % 8 == 0 && 256 % (c / 8) == 0), "bad channel count");
+    switch (which) {
+        case 0: return glue_resources(k_norm_act<false, false>, 256, 0, out);
+        case 1: return glue_resources(k_norm_act<true, false>, 256, (int)((256 / (c / 8)) * kNormRounds * sizeof(TapRec)), out);
+        case 2: return glue_resources(k_norm_act<false, true>, 256, 0, out);
+        case 3: return glue_resources(k_heads, 256, 0, out);
+        case 4: return glue_resources(k_nchw_to_nhwc_split, 256, 0, out);
+    }
+    lwb::set_error("unknown kernel %d", which);
+    return LWB_E_INVALID;
 }

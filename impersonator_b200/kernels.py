@@ -305,6 +305,49 @@ class ConvPlan(object):
             pass
 
 
+# (N tile, operand mode) of the k_conv_wg instances ImpersonatorGenerator.inference launches by default (fp16f8): the
+# row-K stem (fp16x3, swapped 64-channel tiles), every 128-wide N tile, the 128 -> 64 skipper, the folded 7x7 heads
+GENERATOR_CONV_INSTANCES = ((64, 1), (128, 2), (64, 2), (32, 2))
+# the HBM-bound kernels that run beside them on the other sub-batch stream: name -> (lwb_glue_kernel_resources which, c)
+GENERATOR_GLUE_INSTANCES = {"k_norm_act": (0, 0), "k_norm_act<WARP> c=128": (1, 128), "k_norm_act<WARP> c=256": (1, 256),
+                            "k_norm_act<WARP> c=512": (1, 512), "k_heads": (3, 0), "k_nchw_to_nhwc_split": (4, 0)}
+_RES_KEYS = ("regs", "static_smem", "dyn_smem", "local_bytes", "threads", "blocks_alone", "consumer_regs")
+
+
+def conv_kernel_resources(n_tile, mode):
+    """Registers, shared memory and CTAs per SM of one k_conv_wg instance as launched (lwb_conv_kernel_resources)."""
+    out = (ctypes.c_int * 7)()
+    check(lib().lwb_conv_kernel_resources(n_tile, mode, out), "lwb_conv_kernel_resources")
+    return dict(zip(_RES_KEYS, out))
+
+
+def glue_kernel_resources(which, c=0):
+    """The same for k_norm_act (which 0 / 1 = WARP at c channels / 2 = EXT), k_heads (3), k_nchw_to_nhwc_split (4)."""
+    out = (ctypes.c_int * 6)()
+    check(lib().lwb_glue_kernel_resources(which, c, out), "lwb_glue_kernel_resources")
+    return dict(zip(_RES_KEYS, out))
+
+
+def blocks_beside(conv, other, props):
+    """Blocks of ``other`` that fit on an SM that already holds one CTA of ``conv`` (dicts of *_kernel_resources;
+    ``props`` = torch.cuda.get_device_properties).  The rules of the CUDA occupancy calculator (cuda_occupancy.h):
+    registers are allocated per warp in units of 256 from the register file of the warp's sub-partition (four per SM,
+    warp w of a block on sub-partition w % 4), shared memory per block plus 1 KB reserved by the system."""
+    def warp_regs(r):
+        return -(-r * 32 // 256) * 256
+    parts = 4
+    per_part = props.regs_per_multiprocessor // parts
+    conv_warps = conv["threads"] // 32
+    used = [warp_regs(conv["regs"]) * len(range(p, conv_warps, parts)) for p in range(parts)]
+    warps = other["threads"] // 32
+    need = -(-warps // parts) * warp_regs(other["regs"])            # on the sub-partition that gets the most of its warps
+    by_regs = min((per_part - u) // need for u in used)
+    smem = lambda k: k["static_smem"] + k["dyn_smem"] + 1024
+    by_smem = (props.shared_memory_per_multiprocessor - smem(conv)) // smem(other)
+    by_threads = (props.max_threads_per_multi_processor - conv["threads"]) // other["threads"]
+    return max(0, min(by_regs, by_smem, by_threads))
+
+
 def make_conv_desc(n, h_in, w_in, cin0, cout, kh, kw, stride=1, pad=0, dil=1, cin1=0, transposed=False,
                    split=True, rowk=False, row_pitch=0, n_tile=0, halo=False, pad_w=None):
     if transposed:

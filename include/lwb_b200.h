@@ -164,6 +164,10 @@ int  lwb_conv_plan_create(const lwb_conv_desc* d,
 int  lwb_conv_plan_run(const lwb_conv_plan* plan, lwb_stream_t stream);
 int  lwb_conv_plan_num_launches(const lwb_conv_plan* plan);
 void lwb_conv_plan_destroy(lwb_conv_plan* plan);
+/* Resources of the conv kernel instance (n_tile 16/32/64/128, mode = lwb_conv_desc.split) as launched:
+ * out[7] = {registers per thread at launch, static smem, dynamic smem, local bytes per thread, threads per CTA,
+ * CTAs per SM alone, consumer registers per thread after setmaxnreg}.  Needs a device. */
+int  lwb_conv_kernel_resources(int n_tile, int mode, int* out);
 /* create + run + destroy */
 int lwb_conv2d_nhwc(const lwb_conv_desc* d,
                     const uint16_t* x0_hi, const uint16_t* x0_lo,
@@ -205,6 +209,11 @@ int lwb_norm_act_nhwc(const float* raw, const double* stats, const float* gamma,
 int lwb_pack_head_weights(const float* w_img /* [3,64,7,7] */, const float* w_att /* [1,64,7,7] */,
                           float* w4, lwb_stream_t stream);
 int lwb_conv7x7_heads_nhwc(const float* x, const float* w4, int n, int h, int w, float* out, lwb_stream_t stream);
+
+/* Resources of the HBM-bound kernels launched beside the convolutions: which = 0 lwb_norm_act_nhwc (plain),
+ * 1 its warp variant at c channels, 2 its post-affine / strided-residual variant, 3 lwb_heads_composite,
+ * 4 lwb_nchw_to_nhwc_split.  out[6] = the first six entries of lwb_conv_kernel_resources.  Needs a device. */
+int lwb_glue_kernel_resources(int which, int c, int* out);
 
 /* Output heads + composite:  color = tanh(raw[...,0:3]), mask = sigmoid(raw[...,3]),
  * pred = mask*bg + (1-mask)*color   (networks/generator.py:183-184, models/imitator.py:330-331).
