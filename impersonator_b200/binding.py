@@ -1,0 +1,137 @@
+"""Host-side binding of the networks that run on the conv engine (the generator, HMR, the inpaintor, the Mask R-CNN
+detector, LPIPS' AlexNet and InceptionV3): operand buffers, the operand mode, weight packing with one host sync per
+network, conv plans, eval-mode BatchNorm folding and the per-shape stream caches.  Every kernel call goes through the
+``kernels`` module, so that tests can substitute its front-ends."""
+import os
+
+import torch
+
+from . import graph as _graph
+from . import kernels as K
+from ._lib import LwbError
+
+DEFAULT_PRECISION = "fp16f8"
+
+
+def precision_mode():
+    return os.environ.get("LWB_PRECISION", DEFAULT_PRECISION)
+
+
+def split_mode(mod=None):
+    """LWB_PRECISION (or the module's set_precision pin) -> operand split code of the conv engine (lwb_conv_desc.split):
+    fp16x3 = 1: x_hi*w_hi + x_hi*w_lo + x_lo*w_hi, all fp16 (3 MMAs per K step);
+    fp16f8 = 2: x_hi*w_hi in fp16 + (x*w_lo, x_lo*w) in e4m3 at twice the rate (2 MMA-equivalents per K step);
+    fp16   = 0: single pass (not parity-gated)."""
+    mode = (getattr(mod, '_lwb_precision', None) if mod is not None else None) or precision_mode()
+    codes = {"fp16": 0, "fp16x3": 1, "fp16f8": 2}
+    if mode not in codes:
+        raise LwbError("LWB_PRECISION must be fp16x3, fp16f8 or fp16")
+    return codes[mode]
+
+
+class Operands(object):
+    """An NHWC activation: fp16 hi / lo operands of the next conv (lo only when split != 0; none with half=False) and an
+    optional fp32 copy."""
+    __slots__ = ("hi", "lo", "f32")
+
+    def __init__(self, shape, dev, split=1, f32=False, half=True):
+        self.hi = torch.empty(shape, dtype=torch.float16, device=dev) if half else None
+        self.lo = torch.empty(shape, dtype=torch.float16, device=dev) if (half and split) else None
+        self.f32 = torch.empty(shape, dtype=torch.float32, device=dev) if f32 else None
+
+    @property
+    def pair(self):
+        """(hi, lo), the operand argument of K.ConvPlan."""
+        return (self.hi, self.lo)
+
+    def out(self):
+        """The output keywords of the epilogue front-ends."""
+        return dict(y_f32=self.f32, y_hi=self.hi, y_lo=self.lo)
+
+
+def pack_all(items, split):
+    """[(weight, transposed, cout_pad, cin_pad)] -> [PackedWeight]: max|w| of every layer is read back in ONE host sync
+    (it sets the per-layer weight exponent, kernels.weight_exponent), then each layer is packed."""
+    amax = torch.stack([w.abs().max().float() for w, _, _, _ in items]).tolist()
+    return [K.pack_conv_weight(w, transposed=t, cout_pad=co, cin_pad=ci, split=split, absmax=a)
+            for (w, t, co, ci), a in zip(items, amax)]
+
+
+class Conv(object):
+    """One convolution bound to its operands: ``desc``, the raw fp32 NHWC output ``out`` and, after
+    PlanBinder.finalize(), ``plan``."""
+    __slots__ = ("desc", "x", "weight", "cout_pad", "cin_pad", "out", "plan")
+
+
+class PlanBinder(object):
+    """Collects the convolutions of one stream, then packs every weight with one host sync and creates the plans."""
+
+    def __init__(self, dev, split):
+        self.dev, self.split = dev, split
+        self._shared = {}
+        self._convs = []
+
+    def conv(self, weight, x, n, h, w, stride=1, pad=None, pad_w=None, dil=1, cout_pad=None, cin_pad=None, out=None,
+             share=None):
+        """weight OIHW fp32 over operands x = (hi, lo) of [n, h, w, cin_pad or cin]; pad defaults to kh // 2.  The raw
+        output [n, ho, wo, cout_pad or cout] is ``out`` when given, else the buffer shared by every conv of this binder
+        with the same output shape and ``share`` tag when one is given, else a buffer of its own."""
+        cout, cin, kh, kw = weight.shape
+        r = Conv()
+        r.desc = K.make_conv_desc(n, h, w, cin_pad or cin, cout_pad or cout, kh, kw, stride=stride,
+                                  pad=kh // 2 if pad is None else pad, pad_w=pad_w, dil=dil, split=self.split)
+        shape = (n, r.desc.h_out, r.desc.w_out, cout_pad or cout)
+        if out is None and share is not None:
+            out = self._shared.get((shape, share))
+            if out is None:
+                out = self._shared[(shape, share)] = torch.empty(shape, dtype=torch.float32, device=self.dev)
+        r.out = out if out is not None else torch.empty(shape, dtype=torch.float32, device=self.dev)
+        r.x, r.weight, r.cout_pad, r.cin_pad, r.plan = x, weight, cout_pad, cin_pad, None
+        self._convs.append(r)
+        return r
+
+    def finalize(self):
+        """Pack the weights and create every K.ConvPlan; the fp32 source weights are released."""
+        packed = pack_all([(r.weight, False, r.cout_pad, r.cin_pad) for r in self._convs], self.split)
+        for r, wp in zip(self._convs, packed):
+            r.plan = K.ConvPlan(r.desc, r.x, None, wp, r.out, None)
+            r.weight = None
+        self._convs = []
+
+
+def stream_for(owner, cls, key, *args, limit, **kw):
+    """The per-shape stream ``cls(owner, *args, **kw)`` cached under ``key`` in ``owner.__dict__['_lwb_streams']``: the
+    ``limit`` most recently used shapes are kept (each holds its activations, plans and packed weights)."""
+    streams = owner.__dict__.setdefault('_lwb_streams', {})
+    if key in streams:
+        streams[key] = streams.pop(key)                  # most recently used last
+    else:
+        while len(streams) >= limit:
+            streams.pop(next(iter(streams)))
+        streams[key] = cls(owner, *args, **kw)
+    return _graph.pin(streams[key])                      # a CUDA graph being captured keeps what it replays into alive
+
+
+class StreamOwner(object):
+    """Mixin of the nn.Modules that cache streams with stream_for: loading parameters or moving / casting the module
+    (``_apply``) drops them, so the next call rebuilds them from the current weights."""
+
+    def _lwb_invalidate(self):
+        self.__dict__['_lwb_streams'] = {}
+
+    def load_state_dict(self, *args, **kwargs):
+        out = super(StreamOwner, self).load_state_dict(*args, **kwargs)
+        self._lwb_invalidate()
+        return out
+
+    def _apply(self, fn, *args, **kwargs):
+        out = super(StreamOwner, self)._apply(fn, *args, **kwargs)
+        self._lwb_invalidate()
+        return out
+
+
+def bn_affine(weight, bias, mean, var, eps):
+    """Eval-mode BatchNorm as y = x * scale + shift: folded in float64, returned as contiguous fp32 (scale, shift)."""
+    scale = weight.detach().double() / torch.sqrt(var.detach().double() + eps)
+    shift = bias.detach().double() - mean.detach().double() * scale
+    return scale.float().contiguous(), shift.float().contiguous()

@@ -29,6 +29,7 @@ import torch.nn as nn
 
 from . import kernels as K
 from ._lib import LwbError
+from .binding import Operands, PlanBinder, StreamOwner, stream_for
 
 WEIGHTS_FILE = "maskrcnn_resnet50_fpn_coco-bf2d0c1e.pth"
 NUM_CLASSES = 91
@@ -92,7 +93,8 @@ class FrozenBatchNorm2d(nn.Module):
             self.register_buffer(name, torch.full((n,), val))
 
     def affine(self):
-        """x * scale + shift, computed as torchvision's FrozenBatchNorm2d.forward does (eps 1e-5)."""
+        """x * scale + shift, computed as torchvision's FrozenBatchNorm2d.forward does (eps 1e-5).  Not binding.bn_affine:
+        the detector reproduces torchvision's fp32 rsqrt arithmetic, not a float64 fold."""
         scale = self.weight * (self.running_var + 1e-5).rsqrt()
         return scale, self.bias - self.running_mean * scale
 
@@ -176,23 +178,6 @@ def _pad_rows(w, b, rows):
     return wp, bp
 
 
-class _Ops(object):
-    """fp16 hi / lo conv operands with an optional fp32 copy."""
-    __slots__ = ("hi", "lo", "f32")
-
-    def __init__(self, shape, dev, f32=False):
-        self.hi = torch.empty(shape, dtype=torch.float16, device=dev)
-        self.lo = torch.empty(shape, dtype=torch.float16, device=dev)
-        self.f32 = torch.empty(shape, dtype=torch.float32, device=dev) if f32 else None
-
-    @property
-    def pair(self):
-        return (self.hi, self.lo)
-
-    def out(self):
-        return dict(y_f32=self.f32, y_hi=self.hi, y_lo=self.lo)
-
-
 class _DetStream(object):
     """The detector bound to one input size: plans, buffers and folded weights."""
 
@@ -201,22 +186,7 @@ class _DetStream(object):
         scale = min(800.0 / min(h, w), 1333.0 / max(h, w))
         self.ho, self.wo = int(math.floor(h * scale)), int(math.floor(w * scale))
         self.hp, self.wp = int(math.ceil(self.ho / 32.0) * 32), int(math.ceil(self.wo / 32.0) * 32)
-        self.plans = []
-        pend = []
-        raws = {}
-
-        def raw(n, hh, ww, c, tag=""):
-            key = (n, hh, ww, c, tag)
-            if key not in raws:
-                raws[key] = torch.empty((n, hh, ww, c), dtype=torch.float32, device=dev)
-            return raws[key]
-
-        def plan(wt, x, n, hh, ww, stride=1, tag="", pad=None, out=None):
-            cout, cin, kh, kw = wt.shape
-            d = K.make_conv_desc(n, hh, ww, cin, cout, kh, kw, stride=stride, pad=kh // 2 if pad is None else pad, split=SPLIT)
-            rec = dict(desc=d, x=x, w=wt, out=out if out is not None else raw(n, d.h_out, d.w_out, cout, tag))
-            pend.append(rec)
-            return rec
+        plans = PlanBinder(dev, SPLIT)
 
         def folded(conv, bn):
             sc, sh = bn.affine()
@@ -226,7 +196,7 @@ class _DetStream(object):
         self.w1 = body.conv1.weight.detach().float().contiguous()
         self.ss1 = tuple(t.detach().float().contiguous() for t in body.bn1.affine())
         hh, ww = self.hp // 4, self.wp // 4
-        self.x0 = _Ops((1, hh, ww, 64), dev)
+        self.x0 = Operands((1, hh, ww, 64), dev)
         x = self.x0
         self.blocks = []
         feats = []
@@ -238,22 +208,22 @@ class _DetStream(object):
                 ho, wo = (hh - 1) // s + 1, (ww - 1) // s + 1
                 st = dict()
                 w_, b_ = folded(blk.conv1, blk.bn1)
-                st["c1"], st["b1"] = plan(w_, x.pair, 1, hh, ww), b_
-                st["a1"] = _Ops((1, hh, ww, planes), dev)
+                st["c1"], st["b1"] = plans.conv(w_, x.pair, 1, hh, ww, share="main"), b_
+                st["a1"] = Operands((1, hh, ww, planes), dev)
                 w_, b_ = folded(blk.conv2, blk.bn2)
-                st["c2"], st["b2"] = plan(w_, st["a1"].pair, 1, hh, ww, stride=s), b_
-                st["a2"] = _Ops((1, ho, wo, planes), dev)
+                st["c2"], st["b2"] = plans.conv(w_, st["a1"].pair, 1, hh, ww, stride=s, share="main"), b_
+                st["a2"] = Operands((1, ho, wo, planes), dev)
                 w_, b_ = folded(blk.conv3, blk.bn3)
-                st["c3"] = plan(w_, st["a2"].pair, 1, ho, wo)
+                st["c3"] = plans.conv(w_, st["a2"].pair, 1, ho, wo, share="main")
                 if hasattr(blk, "downsample"):
                     wd, bd = folded(blk.downsample[0], blk.downsample[1])
-                    st["ds"] = plan(wd, x.pair, 1, hh, ww, stride=s, tag="ds")
+                    st["ds"] = plans.conv(wd, x.pair, 1, hh, ww, stride=s, share="ds")
                     st["res"] = None
                     b_ = b_ + bd
                 else:
                     st["ds"], st["res"] = None, x.f32
                 st["b3"] = b_.contiguous()
-                st["y"] = _Ops((1, ho, wo, planes * 4), dev, f32=True)
+                st["y"] = Operands((1, ho, wo, planes * 4), dev, f32=True)
                 x = st["y"]
                 hh, ww = ho, wo
                 self.blocks.append(st)
@@ -267,14 +237,14 @@ class _DetStream(object):
             c = feats[i]
             n_, h_, w_, _ = c.f32.shape
             inner, layer = fpn.inner_blocks[i][0], fpn.layer_blocks[i][0]
-            lat = plan(inner.weight.detach().float().contiguous(), c.pair, 1, h_, w_, tag="lat")
-            self.inners[i] = _Ops((1, h_, w_, 256), dev, f32=True)
-            self.P[i] = _Ops((1, h_, w_, 256), dev, f32=True)
-            lp = plan(layer.weight.detach().float().contiguous(), self.inners[i].pair, 1, h_, w_, tag="fpn")
+            lat = plans.conv(inner.weight.detach().float().contiguous(), c.pair, 1, h_, w_, share="lat")
+            self.inners[i] = Operands((1, h_, w_, 256), dev, f32=True)
+            self.P[i] = Operands((1, h_, w_, 256), dev, f32=True)
+            lp = plans.conv(layer.weight.detach().float().contiguous(), self.inners[i].pair, 1, h_, w_, share="fpn")
             self.fpn.append(dict(i=i, lat=lat, lat_b=inner.bias.detach().float().contiguous(), layer=lp,
                                  layer_b=layer.bias.detach().float().contiguous()))
         h5, w5 = self.P[3].f32.shape[1:3]
-        self.P[4] = _Ops((1, (h5 - 1) // 2 + 1, (w5 - 1) // 2 + 1, 256), dev, f32=True)
+        self.P[4] = Operands((1, (h5 - 1) // 2 + 1, (w5 - 1) // 2 + 1, 256), dev, f32=True)
         # RPN
         head = m.rpn.head
         wc = head.conv[0][0]
@@ -285,9 +255,9 @@ class _DetStream(object):
         self.rpn = []
         for l in range(5):
             _, gh, gw, _ = self.P[l].hi.shape
-            t = _Ops((1, gh, gw, 256), dev)
-            cp = plan(wc.weight.detach().float().contiguous(), self.P[l].pair, 1, gh, gw, tag="rpn")
-            hp_ = plan(wh.contiguous(), t.pair, 1, gh, gw, tag="rpnhead")
+            t = Operands((1, gh, gw, 256), dev)
+            cp = plans.conv(wc.weight.detach().float().contiguous(), self.P[l].pair, 1, gh, gw, share="rpn")
+            hp_ = plans.conv(wh.contiguous(), t.pair, 1, gh, gw)
             self.rpn.append(dict(conv=cp, t=t, head=hp_, grid=(gh, gw), stride=(self.hp // gh, self.wp // gw)))
         self.cells = torch.stack([_cell_anchors(s) for s in ANCHOR_SIZES])
         n_cand = sum(min(RPN_TOP, g["grid"][0] * g["grid"][1] * 3) for g in self.rpn)
@@ -301,20 +271,20 @@ class _DetStream(object):
         self.R, self.rgrid = R, (R // 8, 8)
         rh_, rw_ = self.rgrid
         rh = m.roi_heads
-        self.feats7 = _Ops((R, 7, 7, 256), dev, f32=True)
+        self.feats7 = Operands((R, 7, 7, 256), dev, f32=True)
         self.levels7 = torch.zeros(R, dtype=torch.int32, device=dev)
         w6 = rh.box_head.fc6.weight.detach().float().view(1024, 256, 7, 7).permute(0, 2, 3, 1).reshape(1024, 12544, 1, 1)
         f7in = (self.feats7.hi.view(1, rh_, rw_, 12544), self.feats7.lo.view(1, rh_, rw_, 12544))
-        self.fc6 = plan(w6.contiguous(), f7in, 1, rh_, rw_, tag="fc6")
+        self.fc6 = plans.conv(w6.contiguous(), f7in, 1, rh_, rw_)
         self.fc6_b = rh.box_head.fc6.bias.detach().float().contiguous()
-        self.h6 = _Ops((1, rh_, rw_, 1024), dev)
-        self.fc7 = plan(rh.box_head.fc7.weight.detach().float().view(1024, 1024, 1, 1).contiguous(), self.h6.pair, 1, rh_, rw_, tag="fc7")
+        self.h6 = Operands((1, rh_, rw_, 1024), dev)
+        self.fc7 = plans.conv(rh.box_head.fc7.weight.detach().float().view(1024, 1024, 1, 1).contiguous(), self.h6.pair, 1, rh_, rw_)
         self.fc7_b = rh.box_head.fc7.bias.detach().float().contiguous()
-        self.h7 = _Ops((1, rh_, rw_, 1024), dev)
+        self.h7 = Operands((1, rh_, rw_, 1024), dev)
         bp = rh.box_predictor
         wpr, bpr = _pad_rows(torch.cat([bp.cls_score.weight, bp.bbox_pred.weight]).detach().float(),
                              torch.cat([bp.cls_score.bias, bp.bbox_pred.bias]).detach().float(), 464)
-        self.pred = plan(wpr.view(464, 1024, 1, 1).contiguous(), self.h7.pair, 1, rh_, rw_, tag="pred")
+        self.pred = plans.conv(wpr.view(464, 1024, 1, 1).contiguous(), self.h7.pair, 1, rh_, rw_)
         self.pred_b = bpr.contiguous()
         self.pred_out = torch.empty((R, 464), dtype=torch.float32, device=dev)
         nslot = R * (NUM_CLASSES - 1)
@@ -325,34 +295,29 @@ class _DetStream(object):
         # mask head on the <= 100 detections
         D = BOX_DETS
         self.D = D
-        self.feats14 = _Ops((D, 14, 14, 256), dev, f32=True)
+        self.feats14 = Operands((D, 14, 14, 256), dev, f32=True)
         self.levels14 = torch.zeros(D, dtype=torch.int32, device=dev)
         self.mask_convs = []
         src = self.feats14
         for i in range(4):
             cv = rh.mask_head[i][0]
-            dst = _Ops((D, 14, 14, 256), dev)
-            self.mask_convs.append((plan(cv.weight.detach().float().contiguous(), src.pair, D, 14, 14, tag="mask%d" % (i % 2)),
+            dst = Operands((D, 14, 14, 256), dev)
+            self.mask_convs.append((plans.conv(cv.weight.detach().float().contiguous(), src.pair, D, 14, 14, share="mask%d" % (i % 2)),
                                     cv.bias.detach().float().contiguous(), dst))
             src = dst
         mp = m.roi_heads.mask_predictor
         wt = mp.conv5_mask.weight.detach().float().permute(2, 3, 1, 0).reshape(1024, 256, 1, 1)      # [(dy,dx,co), ci]
-        self.deconv = plan(wt.contiguous(), src.pair, D, 14, 14, tag="deconv")
+        self.deconv = plans.conv(wt.contiguous(), src.pair, D, 14, 14)
         self.deconv_b = mp.conv5_mask.bias.detach().float().contiguous()
-        self.m28 = _Ops((D, 28, 28, 256), dev)
+        self.m28 = Operands((D, 28, 28, 256), dev)
         wl, bl = _pad_rows(mp.mask_fcn_logits.weight.detach().float(), mp.mask_fcn_logits.bias.detach().float(), 96)
-        self.mlog = plan(wl.contiguous(), self.m28.pair, D, 28, 28, tag="mlog")
+        self.mlog = plans.conv(wl.contiguous(), self.m28.pair, D, 28, 28)
         self.mlog_b = bl.contiguous()
         self.mask_logits = torch.empty((D, 28, 28), dtype=torch.float32, device=dev)
         self.mask_probs = torch.empty((D, 28, 28), dtype=torch.float32, device=dev)
         self.masks = torch.empty((D, 1, h, w), dtype=torch.float32, device=dev)
         self.out_boxes = torch.empty((D, 4), dtype=torch.float32, device=dev)
-        # weights: one max|w| sync for the whole network, then the plans
-        amax = torch.stack([p["w"].abs().max().float() for p in pend]).tolist()
-        for p, a in zip(pend, amax):
-            wp = K.pack_conv_weight(p["w"], split=SPLIT, absmax=a)
-            p["plan"] = K.ConvPlan(p["desc"], p["x"], None, wp, p["out"], None)
-            p["w"] = None
+        plans.finalize()
         self.ratio = (float(np.float32(h) / np.float32(self.ho)), float(np.float32(w) / np.float32(self.wo)))
 
     def run(self, img):
@@ -361,51 +326,51 @@ class _DetStream(object):
         c1 = K.conv2d_direct_nchw(self.x, self.w1, None, stride=2, pad=3)
         K.det_stem_pool(c1, self.ss1[0], self.ss1[1], self.x0.hi, self.x0.lo)
         for st in self.blocks:
-            st["c1"]["plan"].run()
-            K.det_bias_act(st["c1"]["out"], st["b1"], relu=True, **st["a1"].out())
-            st["c2"]["plan"].run()
-            K.det_bias_act(st["c2"]["out"], st["b2"], relu=True, **st["a2"].out())
-            st["c3"]["plan"].run()
+            st["c1"].plan.run()
+            K.det_bias_act(st["c1"].out, st["b1"], relu=True, **st["a1"].out())
+            st["c2"].plan.run()
+            K.det_bias_act(st["c2"].out, st["b2"], relu=True, **st["a2"].out())
+            st["c3"].plan.run()
             if st["ds"] is not None:
-                st["ds"]["plan"].run()
-            K.det_bias_act(st["c3"]["out"], st["b3"], relu=True, raw2=st["ds"]["out"] if st["ds"] is not None else None,
+                st["ds"].plan.run()
+            K.det_bias_act(st["c3"].out, st["b3"], relu=True, raw2=st["ds"].out if st["ds"] is not None else None,
                            res=st["res"], **st["y"].out())
         for f in self.fpn:
             i = f["i"]
-            f["lat"]["plan"].run()
-            K.det_bias_act(f["lat"]["out"], f["lat_b"], res=self.inners[i + 1].f32 if i < 3 else None, res_half=True,
+            f["lat"].plan.run()
+            K.det_bias_act(f["lat"].out, f["lat_b"], res=self.inners[i + 1].f32 if i < 3 else None, res_half=True,
                            **self.inners[i].out())
-            f["layer"]["plan"].run()
-            K.det_bias_act(f["layer"]["out"], f["layer_b"], **self.P[i].out())
+            f["layer"].plan.run()
+            K.det_bias_act(f["layer"].out, f["layer_b"], **self.P[i].out())
         K.det_bias_act(self.P[3].f32, None, step=2, out_hw=tuple(self.P[4].hi.shape[1:3]), **self.P[4].out())
         for r in self.rpn:
-            r["conv"]["plan"].run()
-            K.det_bias_act(r["conv"]["out"], self.rpn_b, relu=True, **r["t"].out())
-            r["head"]["plan"].run()
-        K.det_rpn([r["head"]["out"][0] for r in self.rpn], [r["stride"] for r in self.rpn], self.cells, self.rpn_head_b, RPN_TOP,
+            r["conv"].plan.run()
+            K.det_bias_act(r["conv"].out, self.rpn_b, relu=True, **r["t"].out())
+            r["head"].plan.run()
+        K.det_rpn([r["head"].out[0] for r in self.rpn], [r["stride"] for r in self.rpn], self.cells, self.rpn_head_b, RPN_TOP,
                   (self.ho, self.wo), RPN_MIN, XFORM_CLIP, self.cand)
         c = self.cand
         self.props = K.det_nms(c["boxes"], c["scores"], c["groups"], c["valid"], RPN_NMS, self.R)
         P4 = [p.f32 for p in self.P[:4]]
         K.det_roi_align(P4, self.props["boxes"], self.props["count"], 7, levels=self.levels7, **self.feats7.out())
-        self.fc6["plan"].run()
-        K.det_bias_act(self.fc6["out"], self.fc6_b, relu=True, **self.h6.out())
-        self.fc7["plan"].run()
-        K.det_bias_act(self.fc7["out"], self.fc7_b, relu=True, **self.h7.out())
-        self.pred["plan"].run()
-        K.det_bias_act(self.pred["out"], self.pred_b, y_f32=self.pred_out.view(self.pred["out"].shape))
+        self.fc6.plan.run()
+        K.det_bias_act(self.fc6.out, self.fc6_b, relu=True, **self.h6.out())
+        self.fc7.plan.run()
+        K.det_bias_act(self.fc7.out, self.fc7_b, relu=True, **self.h7.out())
+        self.pred.plan.run()
+        K.det_bias_act(self.pred.out, self.pred_b, y_f32=self.pred_out.view(self.pred.out.shape))
         K.det_box_candidates(self.pred_out, NUM_CLASSES, self.props["boxes"], self.props["count"], (self.ho, self.wo), BOX_SCORE,
                              BOX_MIN, XFORM_CLIP, self.bcand)
         b = self.bcand
         self.dets = K.det_nms(b["boxes"], b["scores"], b["groups"], b["valid"], BOX_NMS, self.D, m_max=20 * self.R)
         K.det_roi_align(P4, self.dets["boxes"], self.dets["count"], 14, levels=self.levels14, **self.feats14.out())
         for pl, bias, dst in self.mask_convs:
-            pl["plan"].run()
-            K.det_bias_act(pl["out"], bias, relu=True, **dst.out())
-        self.deconv["plan"].run()
-        K.det_d2s_bias_relu(self.deconv["out"], self.deconv_b, y_hi=self.m28.hi, y_lo=self.m28.lo)
-        self.mlog["plan"].run()
-        K.det_mask_probs(self.mlog["out"], self.mlog_b, self.dets["groups"], self.dets["count"], self.mask_logits, self.mask_probs)
+            pl.plan.run()
+            K.det_bias_act(pl.out, bias, relu=True, **dst.out())
+        self.deconv.plan.run()
+        K.det_d2s_bias_relu(self.deconv.out, self.deconv_b, y_hi=self.m28.hi, y_lo=self.m28.lo)
+        self.mlog.plan.run()
+        K.det_mask_probs(self.mlog.out, self.mlog_b, self.dets["groups"], self.dets["count"], self.mask_logits, self.mask_probs)
         K.det_paste_masks(self.mask_probs, self.dets["boxes"], self.dets["count"], self.ratio, (self.h, self.w), self.masks,
                           self.out_boxes)
         return self
@@ -422,7 +387,7 @@ def _cell_anchors(size):
     return (torch.stack([-ws, -hs, ws, hs], dim=1) / 2).round()
 
 
-class MaskRCNN(nn.Module):
+class MaskRCNN(StreamOwner, nn.Module):
     """torchvision's MaskRCNN (resnet50_fpn, 91 classes) in eval mode: same ``state_dict`` keys, CUDA-only forward."""
 
     def __init__(self):
@@ -430,33 +395,17 @@ class MaskRCNN(nn.Module):
         self.backbone = BackboneWithFPN()
         self.rpn = RegionProposalNetwork()
         self.roi_heads = RoIHeads()
-        self.__dict__['_lwb_streams'] = {}
         self.eval()
-
-    def _invalidate(self):
-        self.__dict__['_lwb_streams'] = {}
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         sd = {k: v for k, v in remap_v1(state_dict).items() if not k.endswith("num_batches_tracked")}
-        out = super(MaskRCNN, self).load_state_dict(sd, strict=strict, **kw)
-        self._invalidate()
-        return out
-
-    def _apply(self, fn, *args, **kwargs):
-        out = super(MaskRCNN, self)._apply(fn, *args, **kwargs)
-        self._invalidate()
-        return out
+        return super(MaskRCNN, self).load_state_dict(sd, strict=strict, **kw)
 
     def stream(self, h, w):
         dev = self.backbone.body.conv1.weight.device
         if dev.type != "cuda":
             raise LwbError("the Mask R-CNN detector runs on CUDA only (no CPU fallback): move it with .cuda()")
-        streams = self.__dict__['_lwb_streams']
-        if (h, w) not in streams:
-            while len(streams) >= 2:
-                streams.pop(next(iter(streams)))
-            streams[(h, w)] = _DetStream(self, h, w, dev)
-        return streams[(h, w)]
+        return stream_for(self, _DetStream, (h, w), h, w, dev, limit=2)
 
     def run(self, img):
         """img [3,h,w] in [-1,1] on the model's device -> the stream holding every stage (nothing synchronised)."""

@@ -20,7 +20,7 @@ fallback: without the CUDA library the calls raise.
 
 Extensions over the reference (all optional): source features may have batch 1 while the target
 batch is B (torch's grid_sample cannot broadcast); ``LWB_PRECISION=fp16`` selects the
-single-pass "fast" mode (the default ``fp16f8`` and ``fp16x3`` both meet the 1e-3 parity bar, see _split_mode);
+single-pass "fast" mode (the default ``fp16f8`` and ``fp16x3`` both meet the 1e-3 parity bar, see binding.split_mode);
 the LWB's grid_sample follows the reference's pinned torch 1.2 (align_corners=True), ``LWB_ALIGN_CORNERS=0``
 selects what torch >= 1.3 does for the same flag-less call (kernels.default_align_corners).
 """
@@ -29,12 +29,9 @@ import os
 import torch
 import torch.nn as nn
 
-from . import graph as _graph
 from . import kernels as K
 from ._lib import LwbError
-
-
-DEFAULT_PRECISION = "fp16f8"
+from .binding import Operands, StreamOwner, pack_all, precision_mode, split_mode, stream_for
 
 
 _WEIGHTS_EPOCH = [0]
@@ -50,10 +47,6 @@ def weights_epoch():
     """Bumped whenever a network's parameters may have changed (load_state_dict, init_weights, .to()/.half()...): packed
     weights and per-shape streams are rebuilt then, and anything that cached launches against them must be rebuilt too."""
     return _WEIGHTS_EPOCH[0]
-
-
-def precision_mode():
-    return os.environ.get("LWB_PRECISION", DEFAULT_PRECISION)
 
 
 def _sub_batches(B, enc_w, res_w, bg):
@@ -108,18 +101,6 @@ def fold_head_weights(w_img, w_att):
     return torch.cat([folded, torch.zeros(4, w4.shape[1], 7, 1, dtype=folded.dtype, device=folded.device)], dim=0).contiguous()
 
 
-def _split_mode(mod=None):
-    """LWB_PRECISION -> operand split code of the conv engine (lwb_conv_desc.split):
-    fp16x3 = 1: x_hi*w_hi + x_hi*w_lo + x_lo*w_hi, all fp16 (3 MMAs per K step);
-    fp16f8 = 2: x_hi*w_hi in fp16 + (x*w_lo, x_lo*w) in e4m3 at twice the rate (2 MMA-equivalents per K step);
-    fp16   = 0: single pass (not parity-gated)."""
-    mode = (getattr(mod, '_lwb_precision', None) if mod is not None else None) or precision_mode()
-    codes = {"fp16": 0, "fp16x3": 1, "fp16f8": 2}
-    if mode not in codes:
-        raise LwbError("LWB_PRECISION must be fp16x3, fp16f8 or fp16")
-    return codes[mode]
-
-
 def _align_corners():
     return K.default_align_corners()
 
@@ -133,7 +114,7 @@ def _halo_mode():
     return os.environ.get("LWB_HALO", "0")
 
 
-class NetworkBase(nn.Module):
+class NetworkBase(StreamOwner, nn.Module):
     """networks/networks.py:45-80."""
 
     def __init__(self):
@@ -209,15 +190,6 @@ class NetworkBase(nn.Module):
             out |= int(b)
         return out
 
-    def load_state_dict(self, *args, **kwargs):
-        out = super(NetworkBase, self).load_state_dict(*args, **kwargs)
-        self._lwb_invalidate()
-        return out
-
-    def _apply(self, fn, *args, **kwargs):
-        out = super(NetworkBase, self)._apply(fn, *args, **kwargs)
-        self._lwb_invalidate()
-        return out
 
 
 class ResidualBlock(nn.Module):
@@ -239,20 +211,6 @@ class ResidualBlock(nn.Module):
 # ------------------------------------------------------------------------------------------
 # engine: one network bound to (batch, H, W, precision) -> persistent buffers + conv plans
 # ------------------------------------------------------------------------------------------
-class _Act(object):
-    """An activation: NHWC fp16 hi/lo operands for the next conv, optional fp32 copy."""
-    __slots__ = ("hi", "lo", "f32")
-
-    def __init__(self, shape, dev, split, want_f32=False, want_half=True):
-        self.hi = torch.empty(shape, dtype=torch.float16, device=dev) if want_half else None
-        self.lo = torch.empty(shape, dtype=torch.float16, device=dev) if (want_half and split) else None
-        self.f32 = torch.empty(shape, dtype=torch.float32, device=dev) if want_f32 else None
-
-    @property
-    def pair(self):
-        return (self.hi, self.lo)
-
-
 class _Layer(object):
     """conv (+ InstanceNorm params) bound to buffers: plan + stats slot."""
     __slots__ = ("plan", "raw", "stats", "gamma", "beta", "w", "wsrc")
@@ -314,12 +272,9 @@ class _StreamBase(object):
         self.range_flag = self._zero[nstat * 8:].view(torch.int32)
         self.ws = torch.empty((self.B, cmax, 2), dtype=torch.float32, device=self.dev)
         pend = [L for L in self._layers if L.wsrc is not None]
-        if pend:
-            # per-layer weight exponent of the packing (kernels.weight_exponent): ONE host sync
-            amax = torch.stack([L.wsrc[0].abs().max().float() for L in pend]).tolist()
-            for L, a in zip(pend, amax):
-                L.w = K.pack_conv_weight(L.wsrc[0], transposed=L.wsrc[1], split=self.split, absmax=a)
-                L.wsrc = None
+        packed = pack_all([(L.wsrc[0], L.wsrc[1], None, None) for L in pend], self.split)
+        for L, wp in zip(pend, packed):
+            L.w, L.wsrc = wp, None
         for L in self._layers:
             slot, cout = L.stats
             # per-layer contiguous [B, cout, 2] view at the head of the slot (None: no norm follows)
@@ -360,7 +315,7 @@ class _UnetStream(_StreamBase):
         self.keep_f32 = keep_f32
         # stem input: padded NHWC8 (3 px border top/left/bottom, 5 right) for the row-K 7x7 conv
         self.pitch = W + 8
-        self.x_pad = _Act((B, H + 6, self.pitch, 8), dev, split)
+        self.x_pad = Operands((B, H + 6, self.pitch, 8), dev, split)
         self.cin = net.encoders[0][0].weight.shape[1]
         if self.cin > 8:
             raise LwbError("stem supports at most 8 input channels")
@@ -370,18 +325,18 @@ class _UnetStream(_StreamBase):
         hm = _halo_mode()
         self.enc_layers.append(self._make_layer(net.encoders[0][0], net.encoders[0][1], self.x_pad.pair, rowk=True,
                                                 row_pitch=self.pitch, h=H, w=W, halo=(hm != '0')))
-        self.e.append(_Act((B, h, w, c), dev, split, want_f32=keep_f32))
+        self.e.append(Operands((B, h, w, c), dev, split, f32=keep_f32))
         for i in range(1, nd + 1):
             self.enc_layers.append(self._make_layer(net.encoders[i][0], net.encoders[i][1], self.e[i - 1].pair,
                                                     stride=2, h=h, w=w))
             c, h, w = c * 2, h // 2, w // 2
-            self.e.append(_Act((B, h, w, c), dev, split, want_f32=(keep_f32 or i == nd)))
+            self.e.append(Operands((B, h, w, c), dev, split, f32=(keep_f32 or i == nd)))
         # resnets (ping-pong x buffers; h buffer for the mid activation)
-        self.hb = _Act((B, h, w, c), dev, split)
+        self.hb = Operands((B, h, w, c), dev, split)
         self.res_layers, self.res_out = [], []
         prev = self.e[nd]
         for i in range(self.repeat):
-            out = _Act((B, h, w, c), dev, split, want_f32=True)
+            out = Operands((B, h, w, c), dev, split, f32=True)
             l1 = self._make_layer(net.resnets[i].main[0], net.resnets[i].main[1], prev.pair, h=h, w=w, halo=(hm == 'all'))
             l2 = self._make_layer(net.resnets[i].main[3], net.resnets[i].main[4], self.hb.pair, h=h, w=w, halo=(hm == 'all'))
             self.res_layers.append((l1, l2))
@@ -390,12 +345,12 @@ class _UnetStream(_StreamBase):
         # decoders + skippers
         self.dec_layers, self.d_up, self.d_out = [], [], []
         for i in range(nd):
-            up = _Act((B, h * 2, w * 2, c // 2), dev, split)
+            up = Operands((B, h * 2, w * 2, c // 2), dev, split)
             ld = self._make_layer(net.decoders[i][0], net.decoders[i][1], prev.pair, stride=2, transposed=True, h=h, w=w)
             c, h, w = c // 2, h * 2, w * 2
             last = (i == nd - 1)
             tc_heads = (hm != '0') or (_tc_heads() and c == 64)
-            out = _Act((B, h, w, c), dev, split, want_f32=(last and not tc_heads), want_half=(not last or tc_heads))
+            out = Operands((B, h, w, c), dev, split, f32=(last and not tc_heads), half=(not last or tc_heads))
             ls = self._make_layer(net.skippers[i][0], net.skippers[i][1], self.e[nd - 1 - i].pair, x1=up.pair, h=h, w=w,
                                   halo=(hm != '0'))
             self.dec_layers.append((ld, ls))
@@ -501,27 +456,27 @@ class _ResnetStream(_StreamBase):
         layers = list(net.model)
         nd, rep = net._n_down, net._repeat_num
         self.pitch = W + 8
-        self.x_pad = _Act((B, H + 6, self.pitch, 8), dev, split)
+        self.x_pad = Operands((B, H + 6, self.pitch, 8), dev, split)
         self.cin = layers[0].weight.shape[1]
         if self.cin > 8:
             raise LwbError("stem supports at most 8 input channels")
         self.seq = []
         i = 0
         c, h, w = layers[0].weight.shape[0], H, W
-        out = _Act((B, h, w, c), dev, split)
+        out = Operands((B, h, w, c), dev, split)
         self.seq.append(("cn", self._make_layer(layers[0], layers[1], self.x_pad.pair, rowk=True, row_pitch=self.pitch, h=H, w=W), out, True, None))
         prev = out
         i += 3
         for k in range(nd):
-            out = _Act((B, h // 2, w // 2, c * 2), dev, split, want_f32=(k == nd - 1))
+            out = Operands((B, h // 2, w // 2, c * 2), dev, split, f32=(k == nd - 1))
             self.seq.append(("cn", self._make_layer(layers[i], layers[i + 1], prev.pair, stride=2, h=h, w=w), out, True, None))
             c, h, w = c * 2, h // 2, w // 2
             prev = out
             i += 3
-        hb = _Act((B, h, w, c), dev, split)
+        hb = Operands((B, h, w, c), dev, split)
         for k in range(rep):
             blk = layers[i]
-            out = _Act((B, h, w, c), dev, split, want_f32=True)
+            out = Operands((B, h, w, c), dev, split, f32=True)
             self.seq.append(("cn", self._make_layer(blk.main[0], blk.main[1], prev.pair, h=h, w=w), hb, True, None))
             self.seq.append(("cn", self._make_layer(blk.main[3], blk.main[4], hb.pair, h=h, w=w), out, False, prev))
             prev = out
@@ -529,7 +484,7 @@ class _ResnetStream(_StreamBase):
         for k in range(nd):
             last = (k == nd - 1)
             tc_heads = _tc_heads() and c // 2 == 64
-            out = _Act((B, h * 2, w * 2, c // 2), dev, split, want_f32=(last and not tc_heads), want_half=(not last or tc_heads))
+            out = Operands((B, h * 2, w * 2, c // 2), dev, split, f32=(last and not tc_heads), half=(not last or tc_heads))
             self.seq.append(("cn", self._make_layer(layers[i], layers[i + 1], prev.pair, stride=2, transposed=True, h=h, w=w), out, True, None))
             c, h, w = c // 2, h * 2, w * 2
             prev = out
@@ -581,14 +536,8 @@ def profile_streams(warm_fn, run_fn):
 
 
 def _stream_for(mod, cls, key, *args, **kw):
-    streams = mod.__dict__.setdefault('_lwb_streams', {})
-    if key in streams:
-        streams[key] = streams.pop(key)                  # most recently used last
-    else:
-        while len(streams) >= 8:                         # evict the least recently used shape only (each holds ~GBs at B=16)
-            streams.pop(next(iter(streams)))
-        streams[key] = cls(mod, *args, **kw)
-    return _graph.pin(streams[key])                      # a CUDA graph being captured keeps what it replays into alive
+    """The generator networks' per-shape stream cache: the 8 most recently used shapes (each holds ~GBs at B=16)."""
+    return stream_for(mod, cls, key, *args, limit=8, **kw)
 
 
 def _nhwc_of(t):
@@ -637,7 +586,7 @@ class ResNetGenerator(NetworkBase):
             c = c.expand(c.size(0), c.size(1), x.size(2), x.size(3))
             x = torch.cat([x, c], dim=1)
         B, _, H, W = x.shape
-        split = _split_mode(self)
+        split = split_mode(self)
         st = _stream_for(self, _ResnetStream, ('bg', B, H, W, split), B, H, W, x.device, split)
         return st.run(x)
 
@@ -693,7 +642,7 @@ class ResUnetGenerator(NetworkBase):
 
     def _stream(self, x, keep_f32, tag):
         B, _, H, W = x.shape
-        split = _split_mode(self)
+        split = split_mode(self)
         return _stream_for(self, _UnetStream, (tag, B, H, W, split, keep_f32), B, H, W, x.device, split, keep_f32=keep_f32)
 
     @torch.no_grad()

@@ -20,7 +20,7 @@ _OPEN = []                                                       # pin lists of 
 
 
 def pin(obj):
-    """Called by the per-shape stream caches (generator._stream_for, ...) for every buffer-owning object they hand out: while
+    """Called by the per-shape stream caches (binding.stream_for) for every buffer-owning object they hand out: while
     a CapturedStep is warming up / capturing, the object is also referenced by that step, so that a later LRU eviction from
     the cache cannot free buffers, plans or TMA descriptors the captured graph still replays into."""
     for keep in _OPEN:

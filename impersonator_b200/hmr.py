@@ -23,7 +23,7 @@ import torch.nn as nn
 
 from . import kernels as K
 from ._lib import LwbError
-from .generator import _Act, _split_mode
+from .binding import Operands, PlanBinder, StreamOwner, bn_affine, split_mode, stream_for
 from .smpl import SMPL
 
 
@@ -100,11 +100,8 @@ class ThetaRegressor(nn.Module):
         self.fc_blocks = nn.Sequential(fc_blocks)
 
 
-def _bn_affine(bn):
-    """eval-mode BatchNorm2d as y = x * scale + shift."""
-    scale = (bn.weight.detach().double() / torch.sqrt(bn.running_var.detach().double() + bn.eps))
-    shift = bn.bias.detach().double() - bn.running_mean.detach().double() * scale
-    return scale.float().contiguous(), shift.float().contiguous()
+def _bn_fold(bn):
+    return bn_affine(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
 
 
 class _HmrStream(object):
@@ -119,27 +116,13 @@ class _HmrStream(object):
         blocks = list(r.blocks())
         h = w = 56                                           # 224 -> conv1 s2 -> 112 -> max_pool(3, 2, ceil) -> 56
         self.x0 = torch.empty((B, h, w, 64), dtype=torch.float32, device=dev)
-        pre = _Act((B, h, w, 64), dev, split)                # relu(bn1(x)) of the first block
+        pre = Operands((B, h, w, 64), dev, split)            # relu(bn1(x)) of the first block
         self.pre0 = pre
-        self.pre0_ss = _bn_affine(blocks[0].bn1)
+        self.pre0_ss = _bn_fold(blocks[0].bn1)
         x_f32 = self.x0
         self.steps = []
-        pend, raws = [], {}
+        plans = PlanBinder(dev, split)
         cmax = 2048
-
-        def raw(hh, ww, c, tag=""):
-            key = (hh, ww, c, tag)
-            if key not in raws:
-                raws[key] = torch.empty((B, hh, ww, c), dtype=torch.float32, device=dev)
-            return raws[key]
-
-        def plan(conv, x_pair, hh, ww, stride=1, tag=""):
-            wt = conv.weight.detach()
-            cout, cin, kh, kw = wt.shape
-            d = K.make_conv_desc(B, hh, ww, cin, cout, kh, kw, stride=stride, pad=kh // 2, split=split)
-            rec = dict(desc=d, x=x_pair, w=wt, out=raw(d.h_out, d.w_out, cout, tag))
-            pend.append(rec)
-            return rec
 
         for bi, blk in enumerate(blocks):
             planes = blk.conv1.weight.shape[0]
@@ -147,28 +130,28 @@ class _HmrStream(object):
             ho, wo = h // s, w // s
             nxt = blocks[bi + 1] if bi + 1 < len(blocks) else None
             st = dict(stride=s)
-            st["c1"] = plan(blk.conv1, pre.pair, h, w)
-            a1 = _Act((B, h, w, planes), dev, split)
-            st["a1"], st["ss2"] = a1, _bn_affine(blk.bn2)
-            st["c2"] = plan(blk.conv2, a1.pair, h, w, stride=s)
-            a2 = _Act((B, ho, wo, planes), dev, split)
-            st["a2"], st["ss3"] = a2, _bn_affine(blk.bn3)
-            st["c3"] = plan(blk.conv3, a2.pair, ho, wo)
+            st["c1"] = plans.conv(blk.conv1.weight.detach(), pre.pair, B, h, w, share="main")
+            a1 = Operands((B, h, w, planes), dev, split)
+            st["a1"], st["ss2"] = a1, _bn_fold(blk.bn2)
+            st["c2"] = plans.conv(blk.conv2.weight.detach(), a1.pair, B, h, w, stride=s, share="main")
+            a2 = Operands((B, ho, wo, planes), dev, split)
+            st["a2"], st["ss3"] = a2, _bn_fold(blk.bn3)
+            st["c3"] = plans.conv(blk.conv3.weight.detach(), a2.pair, B, ho, wo, share="main")
             bias = blk.conv3.bias.detach().float()
             if hasattr(blk, 'shortcut'):
                 sc = blk.shortcut[0]
-                rec = plan(sc, pre.pair, h, w, stride=s, tag="shortcut")       # its raw output lives next to conv3's
+                rec = plans.conv(sc.weight.detach(), pre.pair, B, h, w, stride=s, share="shortcut")    # lives next to conv3's output
                 st["sc"] = rec
                 bias = bias + sc.bias.detach().float()
-                st["res"], st["res_step"] = rec["out"], 1
+                st["res"], st["res_step"] = rec.out, 1
             else:
                 st["sc"] = None
                 st["res"], st["res_step"] = x_f32, s           # identity, subsampled by the block's stride (hmr.py:21-36,103)
             st["bias"] = bias.contiguous()
             st["out"] = torch.empty((B, ho, wo, 4 * planes), dtype=torch.float32, device=dev)
             if nxt is not None:
-                st["post"] = _bn_affine(nxt.bn1)
-                pre = _Act((B, ho, wo, 4 * planes), dev, split)
+                st["post"] = _bn_fold(nxt.bn1)
+                pre = Operands((B, ho, wo, 4 * planes), dev, split)
                 st["pre"] = pre
             else:
                 st["post"], st["pre"] = None, None
@@ -176,13 +159,8 @@ class _HmrStream(object):
             h, w = ho, wo
             self.steps.append(st)
         self.final = x_f32
-        self.post_ss = _bn_affine(r.post_bn)
-        # weights: one max|w| sync for the whole encoder, then the plans
-        amax = torch.stack([p["w"].abs().max().float() for p in pend]).tolist()
-        self.plans = []
-        for p, a in zip(pend, amax):
-            wp = K.pack_conv_weight(p["w"], split=split, absmax=a)
-            p["plan"] = K.ConvPlan(p["desc"], p["x"], None, wp, p["out"], None)
+        self.post_ss = _bn_fold(r.post_bn)
+        plans.finalize()
         self.ws = torch.empty((B, cmax, 2), dtype=torch.float32, device=dev)
         self.range_flag = torch.zeros(1, dtype=torch.int32, device=dev)
         reg = net.regressor
@@ -211,15 +189,15 @@ class _HmrStream(object):
         self._affine(self.x0, self.pre0_ss, self.pre0)                                                  # relu(bn1(x)) of layer1.0
         for st in self.steps:
             if st["sc"] is not None:
-                st["sc"]["plan"].run()                                                                  # shortcut(preact)   :101
-            st["c1"]["plan"].run()
-            self._affine(st["c1"]["out"], st["ss2"], st["a1"])                                          # relu(bn2(conv1))   :102
-            st["c2"]["plan"].run()
-            self._affine(st["c2"]["out"], st["ss3"], st["a2"])                                          # relu(bn3(conv2))   :103
-            st["c3"]["plan"].run()
+                st["sc"].plan.run()                                                                     # shortcut(preact)   :101
+            st["c1"].plan.run()
+            self._affine(st["c1"].out, st["ss2"], st["a1"])                                             # relu(bn2(conv1))   :102
+            st["c2"].plan.run()
+            self._affine(st["c2"].out, st["ss3"], st["a2"])                                             # relu(bn3(conv2))   :103
+            st["c3"].plan.run()
             # out = conv3 + bias (+ shortcut bias) + shortcut; operands of the next block = relu(bn1_next(out))     :104-105
             post = st["post"]
-            K.norm_act_nhwc(st["c3"]["out"], None, None, st["bias"], False, self.ws, residual=st["res"], res_step=st["res_step"],
+            K.norm_act_nhwc(st["c3"].out, None, None, st["bias"], False, self.ws, residual=st["res"], res_step=st["res_step"],
                             y_f32=st["out"], y_hi=st["pre"].hi if st["pre"] is not None else None,
                             y_lo=st["pre"].lo if st["pre"] is not None else None, lo_format=self.lo_format,
                             post_scale=post[0] if post else None, post_shift=post[1] if post else None, post_relu=True,
@@ -235,7 +213,7 @@ class _HmrStream(object):
         return theta.clone()
 
 
-class HumanModelRecovery(nn.Module):
+class HumanModelRecovery(StreamOwner, nn.Module):
     def __init__(self, smpl_pkl_path=None, feature_dim=2048, theta_dim=85, iterations=3, smpl_model=None):
         super(HumanModelRecovery, self).__init__()
         self.resnet = preActResNet50()
@@ -244,20 +222,6 @@ class HumanModelRecovery(nn.Module):
         self.theta_dim = theta_dim
         self.regressor = ThetaRegressor(feature_dim + theta_dim, theta_dim, iterations)
         self.iterations = iterations
-        self.__dict__['_lwb_streams'] = {}
-
-    def _invalidate(self):
-        self.__dict__['_lwb_streams'] = {}
-
-    def load_state_dict(self, *args, **kwargs):
-        out = super(HumanModelRecovery, self).load_state_dict(*args, **kwargs)
-        self._invalidate()
-        return out
-
-    def _apply(self, fn, *args, **kwargs):
-        out = super(HumanModelRecovery, self)._apply(fn, *args, **kwargs)
-        self._invalidate()
-        return out
 
     @torch.no_grad()
     def forward(self, inputs):
@@ -267,15 +231,8 @@ class HumanModelRecovery(nn.Module):
         if not inputs.is_cuda:
             raise LwbError("HumanModelRecovery runs on CUDA tensors only (no CPU fallback)")
         B = inputs.shape[0]
-        split = _split_mode(self)
-        streams = self.__dict__['_lwb_streams']
-        key = (B, split)
-        if key not in streams:
-            while len(streams) >= 2:
-                streams.pop(next(iter(streams)))
-            streams[key] = _HmrStream(self, B, inputs.device, split)
-        from . import graph as _graph
-        return _graph.pin(streams[key]).run(inputs)
+        split = split_mode(self)
+        return stream_for(self, _HmrStream, (B, split), B, inputs.device, split, limit=2).run(inputs)
 
     def get_details(self, theta):
         cam = theta[:, 0:3].contiguous()

@@ -22,6 +22,7 @@ import torch.nn as nn
 
 from . import kernels as K
 from ._lib import LwbError
+from .binding import Operands, PlanBinder, StreamOwner, bn_affine, split_mode, stream_for
 
 
 def get_pad(in_, ksize, stride, atrous=1):
@@ -120,7 +121,7 @@ class SelfAttention(nn.Module):
         return (out, attention) if self.with_attn else out
 
 
-class InpaintSANet(torch.nn.Module):
+class InpaintSANet(StreamOwner, torch.nn.Module):
     """networks/inpaintor.py:110-202."""
 
     def __init__(self, c_dim=5):
@@ -167,31 +168,10 @@ class InpaintSANet(torch.nn.Module):
             G(cnum, cnum // 2, 3, 1, padding=get_pad(256, 3, 1)),
             G(cnum // 2, 3, 3, 1, padding=get_pad(256, 3, 1), activation=None))
 
-    def _invalidate(self):
-        self.__dict__['_lwb_streams'] = {}
-
-    def load_state_dict(self, *args, **kwargs):
-        out = super(InpaintSANet, self).load_state_dict(*args, **kwargs)
-        self._invalidate()
-        return out
-
-    def _apply(self, fn, *args, **kwargs):
-        out = super(InpaintSANet, self)._apply(fn, *args, **kwargs)
-        self._invalidate()
-        return out
-
     def _stream(self, x):
-        from .generator import _split_mode
         B, _, H, W = x.shape
-        split = _split_mode(self)
-        streams = self.__dict__.setdefault('_lwb_streams', {})
-        key = (B, H, W, split)
-        if key not in streams:
-            while len(streams) >= 2:
-                streams.pop(next(iter(streams)))
-            streams[key] = _InpaintStream(self, B, H, W, x.device, split)
-        from . import graph as _graph
-        return _graph.pin(streams[key])
+        split = split_mode(self)
+        return stream_for(self, _InpaintStream, (B, H, W, split), B, H, W, x.device, split, limit=2)
 
     @torch.no_grad()
     def forward(self, imgs, masks, only_out=False, only_x=False):
@@ -222,16 +202,14 @@ class _InpaintStream(object):
     folded BatchNorms.  Channel counts (4, 16, 32) below the engine's 64-wide K chunk are zero-padded."""
 
     def __init__(self, net, B, H, W, dev, split):
-        from .generator import _Act
         if H % 4 or W % 4:
             raise LwbError("InpaintSANet needs H, W divisible by 4")
         self.B, self.H, self.W, self.dev, self.split = B, H, W, dev, split
         self.lo_format = 1 if split == 2 else 0
         self.range_flag = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._pend = []
-        self._Act = _Act
+        self._plans = PlanBinder(dev, split)
         self.in_f32 = torch.zeros((B, H, W, 64), dtype=torch.float32, device=dev)         # channels 4..63 stay zero
-        self.x_in = _Act((B, H, W, 64), dev, split)
+        self.x_in = Operands((B, H, W, 64), dev, split)
         self.coarse, h, w = self._chain(list(net.coarse_net), self.x_in, H, W, final_f32=True)
         self.refine, h, w = self._chain(list(net.refine_conv_net), self.x_in, H, W, keep_last_f32=True)
         # self attention on [B, h, w, 128]: stacked 1x1 q / k / v convolution (16 + 16 + 128 = 160 output channels)
@@ -244,19 +222,12 @@ class _InpaintStream(object):
         self.att_gamma = att.gamma.detach().float().contiguous()
         last = self.refine[-1]
         self.att_x = last["y_f32"]
-        self.att_raw = torch.empty((B, h, w, wq.shape[0]), dtype=torch.float32, device=dev)
-        d = K.make_conv_desc(B, h, w, 128, wq.shape[0], 1, 1, pad=0, split=split)
-        self.att_rec = dict(desc=d, x=last["out"].pair, w=wq, cout_pad=wq.shape[0], cin_pad=128, raw=self.att_raw)
-        self._pend.append(self.att_rec)
+        self.att = self._plans.conv(wq, last["out"].pair, B, h, w, pad=0, cout_pad=wq.shape[0], cin_pad=128)
         self.att_out = torch.empty((B, h, w, 128), dtype=torch.float32, device=dev)
-        self.att_act = _Act((B, h, w, 128), dev, split)
+        self.att_act = Operands((B, h, w, 128), dev, split)
         self.upsample, h, w = self._chain(list(net.refine_upsample_net), self.att_act, h, w, final_f32=True)
-        # one max|w| sync for the whole network, then pack + plan
-        amax = torch.stack([p["w"].abs().max().float() for p in self._pend]).tolist()
-        for p, a in zip(self._pend, amax):
-            wp = K.pack_conv_weight(p["w"], cout_pad=p["cout_pad"], cin_pad=p["cin_pad"], split=split, absmax=a)
-            p["plan"] = K.ConvPlan(p["desc"], p["x"], None, wp, p["raw"], None)
-        del self._pend
+        self._plans.finalize()
+        del self._plans
 
     def _chain(self, layers, x_act, h, w, final_f32=False, keep_last_f32=False):
         """Bind a Sequential of gated (de)conv layers.  -> (records, h, w) of the output."""
@@ -271,20 +242,17 @@ class _InpaintStream(object):
             stride, pad, dil = conv.stride[0], conv.padding[0], conv.dilation[0]
             cin_pad = x_act.hi.shape[3]
             wst = torch.cat([conv.weight, g.mask_conv2d.weight], dim=0).detach().float()
-            cout_pad = _ceil_to(2 * cout, 16)
-            d = K.make_conv_desc(B, h, w, cin_pad, cout_pad, k, k, stride=stride, pad=pad, dil=dil, split=split)
-            raw = torch.empty((B, d.h_out, d.w_out, cout_pad), dtype=torch.float32, device=dev)
-            rec = dict(desc=d, x=x_act.pair, w=wst, cout_pad=cout_pad, cin_pad=cin_pad, raw=raw, c=cout)
+            cv = self._plans.conv(wst, x_act.pair, B, h, w, stride=stride, pad=pad, dil=dil, cout_pad=_ceil_to(2 * cout, 16),
+                                  cin_pad=cin_pad)
+            rec = dict(conv=cv, c=cout)
             rec["bias"] = torch.cat([conv.bias, g.mask_conv2d.bias]).detach().float().contiguous() if conv.bias is not None else None
             rec["act"] = 0 if g.activation is None else 2
             if g.batch_norm:
                 bn = g.batch_norm2d
-                sc = (bn.weight.detach().double() / torch.sqrt(bn.running_var.detach().double() + bn.eps))
-                rec["scale"] = sc.float().contiguous()
-                rec["shift"] = (bn.bias.detach().double() - bn.running_mean.detach().double() * sc).float().contiguous()
+                rec["scale"], rec["shift"] = bn_affine(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
             else:
                 rec["scale"] = rec["shift"] = None
-            h, w = d.h_out, d.w_out
+            h, w = cv.desc.h_out, cv.desc.w_out
             last = (i == len(layers) - 1)
             # a GatedDeConv that FOLLOWS consumes this layer's output on the 2x nearest grid (networks/inpaintor.py:67)
             nxt_de = (not last) and isinstance(layers[i + 1], GatedDeConv2dWithActivation)
@@ -292,12 +260,11 @@ class _InpaintStream(object):
             if last and final_f32:
                 rec["out"], rec["y_f32"], rec["clamp"] = None, torch.empty((B, h, w, cout), dtype=torch.float32, device=dev), True
             else:
-                rec["out"] = self._Act((B, h * rec["up"], w * rec["up"], _ceil_to(cout, 64)), dev, split)
+                rec["out"] = Operands((B, h * rec["up"], w * rec["up"], _ceil_to(cout, 64)), dev, split)
                 rec["y_f32"] = torch.empty((B, h, w, cout), dtype=torch.float32, device=dev) if (last and keep_last_f32) else None
                 rec["clamp"] = False
                 x_act = rec["out"]
                 h, w = h * rec["up"], w * rec["up"]
-            self._pend.append(rec)
             recs.append(rec)
         return recs, h, w
 
@@ -311,9 +278,9 @@ class _InpaintStream(object):
 
     def _run_chain(self, recs):
         for r in recs:
-            r["plan"].run()
+            r["conv"].plan.run()
             out = r["out"]
-            K.gated_act_nhwc(r["raw"], r["c"], r["bias"], r["act"], r["scale"], r["shift"], upsample=r["up"], clamp=r["clamp"],
+            K.gated_act_nhwc(r["conv"].out, r["c"], r["bias"], r["act"], r["scale"], r["shift"], upsample=r["up"], clamp=r["clamp"],
                              y_f32=r["y_f32"], y_hi=out.hi if out is not None else None, y_lo=out.lo if out is not None else None,
                              lo_format=self.lo_format, range_flag=self.range_flag)
         return recs[-1]
@@ -327,8 +294,8 @@ class _InpaintStream(object):
     def run_refine(self, x):
         self._load(x)
         self._run_chain(self.refine)
-        self.att_rec["plan"].run()
-        K.self_attention_nhwc(self.att_raw, self.att_bias, self.att_x, self.att_gamma, out=self.att_out)
+        self.att.plan.run()
+        K.self_attention_nhwc(self.att.out, self.att_bias, self.att_x, self.att_gamma, out=self.att_out)
         K.norm_act_nhwc(self.att_out, None, None, None, False, None, y_hi=self.att_act.hi, y_lo=self.att_act.lo,
                         lo_format=self.lo_format, range_flag=self.range_flag)
         last = self._run_chain(self.upsample)

@@ -31,6 +31,7 @@ import torch
 
 from . import kernels as K
 from ._lib import LwbError
+from .binding import Conv, Operands, PlanBinder, bn_affine, stream_for
 
 ALEXNET_FILE = "alexnet-owt-7be5be79.pth"
 LIN_FILE = os.path.join("lpips", "weights", "v0.1", "alex.pth")
@@ -150,11 +151,11 @@ def load_lin_weights(lin_weights=None):
 class _AlexStream(object):
     """AlexNet features + LPIPS taps bound to (N pairs, H, W): buffers, conv plans and weights on the device."""
 
-    def __init__(self, convs, lins, n, h, w, dev):
+    def __init__(self, owner, n, h, w, dev):
         self.n, self.h, self.w = n, h, w
+        convs, lins = owner.convs, owner.lins
         n2 = 2 * n
         f = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
-        ops = lambda *s: (torch.empty(s, dtype=torch.float16, device=dev), torch.empty(s, dtype=torch.float16, device=dev))
         self.x = f(n2, 3, h, w)
         self.w1 = convs[0][0].to(dev).contiguous()
         self.b1 = convs[0][1].to(dev).contiguous()
@@ -164,21 +165,18 @@ class _AlexStream(object):
         if min(h1, w1) < 3 or min(hp1, wp1) < 3 or min(hp2, wp2) < 1:
             raise LwbError("LPIPS: %dx%d frames are too small for AlexNet's features" % (h, w))
         self.feats = [f(n2, h1, w1, 64), f(n2, hp1, wp1, 192), f(n2, hp2, wp2, 384), f(n2, hp2, wp2, 256), f(n2, hp2, wp2, 256)]
-        self.pool1, self.pool2 = ops(n2, hp1, wp1, 64), ops(n2, hp2, wp2, 192)
-        self.a3, self.a4 = ops(n2, hp2, wp2, 384), ops(n2, hp2, wp2, 256)
+        self.pool1, self.pool2 = Operands((n2, hp1, wp1, 64), dev, SPLIT), Operands((n2, hp2, wp2, 192), dev, SPLIT)
+        self.a3, self.a4 = Operands((n2, hp2, wp2, 384), dev, SPLIT), Operands((n2, hp2, wp2, 256), dev, SPLIT)
         ins = (self.pool1, self.pool2, self.a3, self.a4)
         outs = (None, None, self.a3, self.a4, None)
-        amax = torch.stack([c[0].abs().max() for c in convs[1:]]).tolist()
+        plans = PlanBinder(dev, SPLIT)
         self.layers = []
         for k in range(1, 5):
-            _, cin, cout, ks, _, pad = ALEX_CONVS[k]
-            x_pair = ins[k - 1]
-            hh, ww = x_pair[0].shape[1:3]
-            d = K.make_conv_desc(n2, hh, ww, cin, cout, ks, ks, pad=pad, split=SPLIT)
-            raw = f(n2, d.h_out, d.w_out, cout)
-            wp = K.pack_conv_weight(convs[k][0].to(dev), split=SPLIT, absmax=amax[k - 1])
-            plan = K.ConvPlan(d, x_pair, None, wp, raw, None)
-            self.layers.append(dict(plan=plan, raw=raw, bias=convs[k][1].to(dev).contiguous(), out=outs[k]))
+            pad = ALEX_CONVS[k][5]
+            hh, ww = ins[k - 1].hi.shape[1:3]
+            conv = plans.conv(convs[k][0].to(dev), ins[k - 1].pair, n2, hh, ww, pad=pad)
+            self.layers.append(dict(conv=conv, bias=convs[k][1].to(dev).contiguous(), out=outs[k]))
+        plans.finalize()
         self.lins = [l.to(dev).contiguous() for l in lins]
         self.layer_vals = torch.empty((n, 5), dtype=torch.float32, device=dev)
         self.score = torch.empty(n, dtype=torch.float32, device=dev)
@@ -187,14 +185,14 @@ class _AlexStream(object):
         """-> (score [N], per-layer values [N,5]) device views, valid until the next run."""
         K.lpips_input(pred, ref, from01=from01, out=self.x)
         K.conv2d_direct_relu_nhwc(self.x, self.w1, self.b1, stride=4, pad=2, out=self.feats[0])
-        K.maxpool_nhwc(self.feats[0], 3, 2, y_hi=self.pool1[0], y_lo=self.pool1[1])
+        K.maxpool_nhwc(self.feats[0], 3, 2, y_hi=self.pool1.hi, y_lo=self.pool1.lo)
         for k, L in enumerate(self.layers):
-            L["plan"].run()
+            L["conv"].plan.run()
             o = L["out"]
-            K.det_bias_act(L["raw"], L["bias"], relu=True, y_f32=self.feats[k + 1], y_hi=o[0] if o else None,
-                           y_lo=o[1] if o else None)
+            K.det_bias_act(L["conv"].out, L["bias"], relu=True, y_f32=self.feats[k + 1], y_hi=o.hi if o else None,
+                           y_lo=o.lo if o else None)
             if k == 0:
-                K.maxpool_nhwc(self.feats[1], 3, 2, y_hi=self.pool2[0], y_lo=self.pool2[1])
+                K.maxpool_nhwc(self.feats[1], 3, 2, y_hi=self.pool2.hi, y_lo=self.pool2.lo)
         for k in range(5):
             K.lpips_layer(self.feats[k], self.lins[k], k, self.layer_vals, self.score)
         return self.score, self.layer_vals
@@ -207,7 +205,6 @@ class LPIPS(object):
         self.device = _device(device)
         self.convs = load_alexnet_weights(weights)
         self.lins = load_lin_weights(lin_weights)
-        self._streams = {}
 
     def __call__(self, pred, ref, from01=True):
         """-> (per-frame score [N] fp32, per-layer values [N,5]) device tensors (fresh copies)."""
@@ -215,13 +212,8 @@ class LPIPS(object):
         if p.shape != r.shape:
             raise LwbError("pred %s and ref %s differ in shape" % (tuple(p.shape), tuple(r.shape)))
         n, _, h, w = p.shape
-        key = (n, h, w)
         with torch.cuda.device(self.device):
-            st = self._streams.get(key)
-            if st is None:
-                while len(self._streams) >= 2:
-                    self._streams.pop(next(iter(self._streams)))
-                st = self._streams[key] = _AlexStream(self.convs, self.lins, n, h, w, self.device)
+            st = stream_for(self, _AlexStream, (n, h, w), n, h, w, self.device, limit=2)
             score, layers = st.run(p, r, from01)
             return score.clone(), layers.clone()
 
@@ -355,10 +347,8 @@ def load_inception_weights(weights=None):
             t = sd.get("%s.bn.%s" % (name, k))
             if t is None or tuple(t.shape) != (cout,):
                 raise LwbError("InceptionV3 state dict: %s.bn.%s must hold %d values" % (name, k, cout))
-            bn.append(t.double())
-        gamma, beta, mean, var = bn
-        scale = gamma / torch.sqrt(var + BN_EPS)
-        out[name] = (w.float(), scale.float(), (beta - mean * scale).float())
+            bn.append(t)
+        out[name] = (w.float(),) + bn_affine(*bn, BN_EPS)
     return out
 
 
@@ -377,22 +367,23 @@ class _InceptionStream(object):
     def __init__(self, net, n, h, w, dev):
         self.n, self.dev, self.net = n, dev, net
         self.ops = []
+        self._plans = PlanBinder(dev, SPLIT)
         self.x = self._f32(n, 3, 299, 299)
         # Conv2d_1a (BN folded into the fp32 stem) -> operands of 64 channels
         self.stem = self._f32(n, 149, 149, 32)
         self.ops.append(lambda: K.conv2d_direct_relu_nhwc(self.x, net.stem_w, net.stem_b, stride=2, out=self.stem))
-        a = self._ops(n, 149, 149, 64)
+        a = Operands((n, 149, 149, 64), self.dev, SPLIT)
         self._seg(self.stem, 0, None, a, 0, relu=False, c=32, c_out=64)
         a = self._single("Conv2d_2a_3x3", a)
         b2 = self._f32(n, 147, 147, 64)
         self._single("Conv2d_2b_3x3", a, f32=b2)
-        a = self._ops(n, 73, 73, 64)
-        self.ops.append(functools.partial(K.maxpool_nhwc, b2, 3, 2, y_hi=a[0], y_lo=a[1]))
+        a = Operands((n, 73, 73, 64), self.dev, SPLIT)
+        self.ops.append(functools.partial(K.maxpool_nhwc, b2, 3, 2, y_hi=a.hi, y_lo=a.lo))
         a = self._single("Conv2d_3b_1x1", a)
         b4 = self._f32(n, 71, 71, 192)
         self._single("Conv2d_4a_3x3", a, f32=b4)
-        a = self._ops(n, 35, 35, 192)
-        self.ops.append(functools.partial(K.maxpool_nhwc, b4, 3, 2, y_hi=a[0], y_lo=a[1]))
+        a = Operands((n, 35, 35, 192), self.dev, SPLIT)
+        self.ops.append(functools.partial(K.maxpool_nhwc, b4, 3, 2, y_hi=a.hi, y_lo=a.lo))
         a = self._block_a("Mixed_5b", a)
         a = self._block_a("Mixed_5c", a)
         self.mixed_5d = self._f32(n, 35, 35, 320)
@@ -406,13 +397,13 @@ class _InceptionStream(object):
         a = self._block_e("Mixed_7b", a)
         self.feats = self._f32(n, 2048)
         self._block_e("Mixed_7c", a, feats=self.feats)
+        self._plans.finalize()
+        del self._plans
+        self.ops = [op.plan.run if isinstance(op, Conv) else op for op in self.ops]
 
     # -- buffers and launches --
     def _f32(self, *s):
         return torch.empty(s, dtype=torch.float32, device=self.dev)
-
-    def _ops(self, *s):
-        return (torch.empty(s, dtype=torch.float16, device=self.dev), torch.empty(s, dtype=torch.float16, device=self.dev))
 
     def _conv(self, names, x):
         """One conv-engine GEMM of the same-input, same-shape convolutions ``names`` over operands x [n,h,w,64k]
@@ -421,19 +412,15 @@ class _InceptionStream(object):
         _, _, kh, kw, s, ph, pw = specs[0]
         if any(sp[2:] != specs[0][2:] for sp in specs):
             raise LwbError("merged convolutions must share kernel, stride and padding: %s" % (names,))
-        n, h, w, cp = x[0].shape
+        n, h, w, cp = x.hi.shape
         cols, c0 = {}, 0
         for nm, sp in zip(names, specs):
             cols[nm] = c0
             c0 += sp[1]
-        cout_pad = _up64(c0)
         wt = torch.cat([self.net.convs[nm][0] for nm in names], 0).to(self.dev)
-        wp = K.pack_conv_weight(wt, cout_pad=cout_pad, cin_pad=cp, split=SPLIT)
-        d = K.make_conv_desc(n, h, w, cp, cout_pad, kh, kw, stride=s, pad=ph, pad_w=pw, split=SPLIT)
-        raw = self._f32(n, d.h_out, d.w_out, cout_pad)
-        plan = K.ConvPlan(d, x, None, wp, raw, None)
-        self.ops.append(plan.run)
-        return raw, cols
+        conv = self._plans.conv(wt, x.pair, n, h, w, stride=s, pad=ph, pad_w=pw, cout_pad=_up64(c0), cin_pad=cp)
+        self.ops.append(conv)                            # its plan.run once finalize() has made the plan
+        return conv.out, cols
 
     def _seg(self, raw, c0, name, y, off, relu=True, c=None, c_out=None, box=False, f32=None):
         """Branch ``name`` (columns c0.. of raw) -> BN + ReLU into channels off.. of operands y and / or fp32 f32."""
@@ -442,7 +429,7 @@ class _InceptionStream(object):
             _, scale, shift = self.net.convs[name]
             scale, shift = scale.to(self.dev), shift.to(self.dev)
             c = INCEPTION_CONVS[name][1]
-        hi, lo = y if y is not None else (None, None)
+        hi, lo = y.pair if y is not None else (None, None)
         self.ops.append(lambda: K.bn_act_segment(raw, c0, c, scale, shift, relu=relu, box=box, c_out=c_out, y_f32=f32,
                                                  y_hi=hi, y_lo=lo, off_y=off))
 
@@ -454,7 +441,7 @@ class _InceptionStream(object):
         c_out = cout
         if y is None and f32 is None:
             c_out = _up64(cout)
-            y = self._ops(*raw.shape[:3], c_out)
+            y = Operands((*raw.shape[:3], c_out), self.dev, SPLIT)
         self._seg(raw, 0, name, y, off, c_out=c_out, f32=f32)
         return y
 
@@ -466,12 +453,12 @@ class _InceptionStream(object):
 
     # -- the Inception blocks (torchvision inception.py InceptionA..E) --
     def _block_a(self, b, x, f32=None):
-        n, h, w, _ = x[0].shape
+        n, h, w, _ = x.hi.shape
         raw, col = self._conv([b + ".branch1x1", b + ".branch5x5_1", b + ".branch3x3dbl_1", b + ".branch_pool"], x)
         pf = INCEPTION_CONVS[b + ".branch_pool"][1]
         pitch = _up64(224 + pf)
-        out = self._ops(n, h, w, pitch)
-        t5, td = self._ops(n, h, w, 64), self._ops(n, h, w, 64)
+        out = Operands((n, h, w, pitch), self.dev, SPLIT)
+        t5, td = Operands((n, h, w, 64), self.dev, SPLIT), Operands((n, h, w, 64), self.dev, SPLIT)
         self._seg(raw, col[b + ".branch1x1"], b + ".branch1x1", out, 0, f32=f32)
         self._seg(raw, col[b + ".branch5x5_1"], b + ".branch5x5_1", t5, 0, c_out=64)
         self._seg(raw, col[b + ".branch3x3dbl_1"], b + ".branch3x3dbl_1", td, 0)
@@ -482,21 +469,21 @@ class _InceptionStream(object):
         return out
 
     def _block_b(self, b, x, x_f32, cin):
-        n = x[0].shape[0]
-        out = self._ops(n, 17, 17, 768)
+        n = x.hi.shape[0]
+        out = Operands((n, 17, 17, 768), self.dev, SPLIT)
         self._single(b + ".branch3x3", x, y=out, off=0)
         t = self._single(b + ".branch3x3dbl_1", x)
         t = self._single(b + ".branch3x3dbl_2", t)
         self._single(b + ".branch3x3dbl_3", t, y=out, off=384)
-        self.ops.append(lambda: K.maxpool_nhwc_slice(x_f32, cin, 3, 2, y_hi=out[0], y_lo=out[1], off_y=480))
+        self.ops.append(lambda: K.maxpool_nhwc_slice(x_f32, cin, 3, 2, y_hi=out.hi, y_lo=out.lo, off_y=480))
         return out
 
     def _block_c(self, b, x, f32=None):
-        n, h, w, _ = x[0].shape
+        n, h, w, _ = x.hi.shape
         raw, col = self._conv([b + ".branch1x1", b + ".branch7x7_1", b + ".branch7x7dbl_1", b + ".branch_pool"], x)
         c7 = INCEPTION_CONVS[b + ".branch7x7_1"][1]
-        out = self._ops(n, h, w, 768)
-        ta, tb = self._ops(n, h, w, _up64(c7)), self._ops(n, h, w, _up64(c7))
+        out = Operands((n, h, w, 768), self.dev, SPLIT)
+        ta, tb = Operands((n, h, w, _up64(c7)), self.dev, SPLIT), Operands((n, h, w, _up64(c7)), self.dev, SPLIT)
         self._seg(raw, col[b + ".branch1x1"], b + ".branch1x1", out, 0, f32=f32)
         self._seg(raw, col[b + ".branch7x7_1"], b + ".branch7x7_1", ta, 0, c_out=_up64(c7))
         self._seg(raw, col[b + ".branch7x7dbl_1"], b + ".branch7x7dbl_1", tb, 0, c_out=_up64(c7))
@@ -509,30 +496,30 @@ class _InceptionStream(object):
         return out
 
     def _block_d(self, b, x, x_f32):
-        n = x[0].shape[0]
+        n = x.hi.shape[0]
         raw, col = self._conv([b + ".branch3x3_1", b + ".branch7x7x3_1"], x)
-        out = self._ops(n, 8, 8, 1280)
-        ta, tb = self._ops(n, 17, 17, 192), self._ops(n, 17, 17, 192)
+        out = Operands((n, 8, 8, 1280), self.dev, SPLIT)
+        ta, tb = Operands((n, 17, 17, 192), self.dev, SPLIT), Operands((n, 17, 17, 192), self.dev, SPLIT)
         self._seg(raw, col[b + ".branch3x3_1"], b + ".branch3x3_1", ta, 0)
         self._seg(raw, col[b + ".branch7x7x3_1"], b + ".branch7x7x3_1", tb, 0)
         self._single(b + ".branch3x3_2", ta, y=out, off=0)
         tb = self._single(b + ".branch7x7x3_2", tb)
         tb = self._single(b + ".branch7x7x3_3", tb)
         self._single(b + ".branch7x7x3_4", tb, y=out, off=320)
-        self.ops.append(lambda: K.maxpool_nhwc_slice(x_f32, 768, 3, 2, y_hi=out[0], y_lo=out[1], off_y=512))
+        self.ops.append(lambda: K.maxpool_nhwc_slice(x_f32, 768, 3, 2, y_hi=out.hi, y_lo=out.lo, off_y=512))
         return out
 
     def _block_e(self, b, x, feats=None):
-        n, h, w, _ = x[0].shape
+        n, h, w, _ = x.hi.shape
         raw, col = self._conv([b + ".branch1x1", b + ".branch3x3_1", b + ".branch3x3dbl_1", b + ".branch_pool"], x)
-        ta, tb = self._ops(n, h, w, 384), self._ops(n, h, w, 448)
+        ta, tb = Operands((n, h, w, 384), self.dev, SPLIT), Operands((n, h, w, 448), self.dev, SPLIT)
         self._seg(raw, col[b + ".branch3x3_1"], b + ".branch3x3_1", ta, 0)
         self._seg(raw, col[b + ".branch3x3dbl_1"], b + ".branch3x3dbl_1", tb, 0)
         tc = self._single(b + ".branch3x3dbl_2", tb)
         branches = ((ta, "branch3x3_2a", 320), (ta, "branch3x3_2b", 704), (tc, "branch3x3dbl_3a", 1088),
                     (tc, "branch3x3dbl_3b", 1472))
         if feats is None:
-            out = self._ops(n, h, w, 2048)
+            out = Operands((n, h, w, 2048), self.dev, SPLIT)
             self._seg(raw, col[b + ".branch1x1"], b + ".branch1x1", out, 0)
             self._seg(raw, col[b + ".branch_pool"], b + ".branch_pool", out, 1856, box=True)
             for src, nm, off in branches:
@@ -568,16 +555,9 @@ class InceptionFeatures(object):
         self.stem_w = (w.double() * scale.double().view(-1, 1, 1, 1)).float().to(self.device).contiguous()
         self.stem_b = shift.to(self.device).contiguous()
         self.convs = convs
-        self._streams = {}
 
     def stream(self, n, h, w):
-        key = (n, h, w)
-        st = self._streams.get(key)
-        if st is None:
-            while len(self._streams) >= 2:
-                self._streams.pop(next(iter(self._streams)))
-            st = self._streams[key] = _InceptionStream(self, n, h, w, self.device)
-        return st
+        return stream_for(self, _InceptionStream, (n, h, w), n, h, w, self.device, limit=2)
 
     def __call__(self, frames):
         """-> fresh [N, 2048] fp32 CUDA tensor."""

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY -- torch-CPU stand-ins for the C-ABI front-ends of impersonator_b200.kernels.
 
-The host mirrors (generator / hmr / inpaintor streams) are pure orchestration: they bind buffers, fold BatchNorms, stack
-gated filters, fold the 7x7 heads into a 7x1 filter, chain conv plans and epilogues.  None of that needs a GPU to be
+The host mirrors (generator / hmr / inpaintor / LPIPS / Inception streams) are pure orchestration: they bind buffers,
+fold BatchNorms, stack gated filters, fold the 7x7 heads into a 7x1 filter, chain conv plans and epilogues.  None of that needs a GPU to be
 wrong.  ``install(monkeypatch)`` replaces every kernel front-end the streams call by a plain torch implementation of the
 SAME contract (include/lwb_b200.h), so the CPU suite can run the whole host logic against the oracles.  The emulation
 works on the fp16 hi/lo operand pairs (run it with LWB_PRECISION=fp16x3); it is never used by the product.
@@ -307,6 +307,102 @@ def warp_nchw(x, T, align_corners=None, out=None, accumulate=False):
     return y
 
 
+def _store(y, y_f32, y_hi, y_lo, off=0):
+    """y -> channels [off, off + y.shape[-1]) of the outputs; the other channels are left alone."""
+    c = y.shape[-1]
+    if y_f32 is not None:
+        y_f32[..., off:off + c] = y
+    if y_hi is not None:
+        hi = y.half()
+        y_hi[..., off:off + c] = hi
+        if y_lo is not None:
+            y_lo[..., off:off + c] = (y - hi.float()).half()
+
+
+def det_bias_act(raw, bias=None, relu=False, raw2=None, res=None, res_half=False, step=1, out_hw=None, c=None,
+                 y_f32=None, y_hi=None, y_lo=None):
+    n, h_in, w_in, ld = raw.shape
+    c = c or ld
+    h, w = out_hw or (h_in, w_in)
+    v = raw[:, ::step, ::step, :c][:, :h, :w]
+    if raw2 is not None:
+        v = v + raw2[:, ::step, ::step, :c][:, :h, :w]
+    if bias is not None:
+        v = v + bias[:c]
+    if res is not None:
+        if res_half:
+            v = v + res.reshape(n, h // 2, w // 2, c).repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
+        else:
+            v = v + res.reshape(n, h, w, c)
+    if relu:
+        v = F.relu(v)
+    _store(v, None if y_f32 is None else y_f32.view(n, h, w, c), y_hi, y_lo)
+
+
+def conv2d_direct_relu_nhwc(x, w, bias=None, stride=1, pad=0, out=None):
+    y = F.relu(F.conv2d(x, w, bias, stride=stride, padding=pad)).permute(0, 2, 3, 1)
+    if out is None:
+        return y.contiguous()
+    out.copy_(y)
+    return out
+
+
+def maxpool_nhwc(x, k, stride, y_f32=None, y_hi=None, y_lo=None):
+    y = F.max_pool2d(x.permute(0, 3, 1, 2), k, stride).permute(0, 2, 3, 1)
+    if y_f32 is None and y_hi is None:
+        return y.contiguous()
+    _store(y, y_f32, y_hi, y_lo)
+    return y_f32
+
+
+def maxpool_nhwc_slice(x, c, k, stride, y_f32=None, y_hi=None, y_lo=None, off_y=0):
+    _store(F.max_pool2d(x[..., :c].permute(0, 3, 1, 2), k, stride).permute(0, 2, 3, 1), y_f32, y_hi, y_lo, off_y)
+
+
+def bn_act_segment(raw, c0, c, scale=None, shift=None, relu=True, box=False, c_out=None, y_f32=None, y_hi=None, y_lo=None,
+                   off_y=0):
+    r = raw[..., c0:c0 + c]
+    if box:
+        r = F.avg_pool2d(r.permute(0, 3, 1, 2), 3, 1, 1, count_include_pad=True).permute(0, 2, 3, 1)
+    v = r * scale + shift if scale is not None else r
+    if relu:
+        v = F.relu(v)
+    _store(F.pad(v, (0, (c_out or c) - c)), y_f32, y_hi, y_lo, off_y)
+
+
+_LPIPS_SHIFT, _LPIPS_SCALE = (-.030, -.088, -.188), (.458, .448, .450)
+
+
+def lpips_input(pred, ref, from01=False, out=None):
+    x = torch.cat([pred, ref])
+    if from01:
+        x = x * 2 - 1
+    shift = torch.tensor(_LPIPS_SHIFT, dtype=torch.float32).view(1, 3, 1, 1)
+    scale = torch.tensor(_LPIPS_SCALE, dtype=torch.float32).view(1, 3, 1, 1)
+    y = (x - shift) / scale
+    if out is None:
+        return y
+    out.copy_(y)
+    return out
+
+
+def lpips_layer(feat, lin, layer, layers, score):
+    n = feat.shape[0] // 2
+    f = feat.double()
+    f = f / (f.pow(2).sum(-1, keepdim=True).sqrt() + 1e-10)
+    v = ((f[n:] - f[:n]) ** 2 * lin.double()).sum(-1).mean(dim=(1, 2)).float()
+    layers[:, layer] = v
+    score.copy_(v if layer == 0 else score + v)
+
+
+def inception_input(x, out=None):
+    y = F.interpolate(x * 2 - 1, size=(299, 299), mode='bilinear', align_corners=False)
+    if out is None:
+        return y
+    out.copy_(y)
+    return out
+
+
 def install_tasks(monkeypatch):
     """install() + the correspondence / warp front-ends and the renderer's CUDA-only guard: enough to run the task classes'
     personalize / view / swap on CPU (Imitator.inference itself drives CUDA streams and stays GPU-only)."""
@@ -326,6 +422,8 @@ def install_tasks(monkeypatch):
 def install(monkeypatch):
     for name in ("pack_conv_weight", "pack_conv_weight_rowk", "ConvPlan", "norm_act_nhwc", "nchw_to_nhwc_split", "nhwc_to_nchw",
                  "conv2d_direct_nchw", "gated_bn_nchw", "gated_act_nhwc", "self_attention_nhwc", "maxpool_nchw_to_nhwc",
-                 "global_avgpool_nhwc", "linear", "pack_head_weights", "conv7x7_heads_nhwc", "heads_composite"):
+                 "global_avgpool_nhwc", "linear", "pack_head_weights", "conv7x7_heads_nhwc", "heads_composite",
+                 "det_bias_act", "conv2d_direct_relu_nhwc", "maxpool_nhwc", "maxpool_nhwc_slice", "bn_act_segment",
+                 "lpips_input", "lpips_layer", "inception_input"):
         monkeypatch.setattr(K, name, globals()[name])
     monkeypatch.setenv("LWB_PRECISION", "fp16x3")

@@ -61,13 +61,13 @@ def _nhwc(t):
     return t[0].permute(1, 2, 0)
 
 
-def test_continuous_stages(run256):
+def test_continuous_stages_match_oracle(run256):
     _, det, st, g = run256
     errs = {}
     for i in range(5):
         errs["P%d" % (i + 2)] = _rel(g.P[i].f32[0].cpu(), _nhwc(st["P"][i]))
     for l, lv in enumerate(st["rpn"]["levels"]):
-        raw = g.rpn[l]["head"]["out"][0].cpu() + g.rpn_head_b.cpu()
+        raw = g.rpn[l]["head"].out[0].cpu() + g.rpn_head_b.cpu()
         gh, gw = raw.shape[:2]
         errs["rpn_logits%d" % l] = _rel(raw[..., :3].reshape(-1), lv["logits"])
         errs["rpn_deltas%d" % l] = _rel(raw[..., 3:15].reshape(-1, 4), lv["deltas"])
