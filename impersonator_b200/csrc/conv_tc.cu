@@ -51,6 +51,7 @@
 
 #include <algorithm>
 #include <new>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -626,24 +627,30 @@ int launch_wg(const Launch& L, cudaStream_t st)
     return LWB_OK;
 }
 
-template <int N_TILE>
-int launch_one(const Launch& L, cudaStream_t st)
+// The one list of k_conv_wg instances: calls f(N_TILE, MODE), both std::integral_constant, for an N tile of 16, 32, 64
+// or 128 and an operand mode.
+template <class F>
+int with_instance(int n_tile, int mode, F&& f)
 {
-    if (L.mode == MODE_F8) return launch_wg<N_TILE, MODE_F8>(L, st);
-    if (L.mode == MODE_FP16X3) return launch_wg<N_TILE, MODE_FP16X3>(L, st);
-    return launch_wg<N_TILE, MODE_FP16>(L, st);
+    auto modes = [&](auto nt) {
+        if (mode == MODE_F8) return f(nt, std::integral_constant<int, MODE_F8>());
+        if (mode == MODE_FP16X3) return f(nt, std::integral_constant<int, MODE_FP16X3>());
+        return f(nt, std::integral_constant<int, MODE_FP16>());
+    };
+    switch (n_tile) {
+        case 16:  return modes(std::integral_constant<int, 16>());
+        case 32:  return modes(std::integral_constant<int, 32>());
+        case 64:  return modes(std::integral_constant<int, 64>());
+        case 128: return modes(std::integral_constant<int, 128>());
+    }
+    lwb::set_error("conv_tc: unsupported N tile %d", n_tile);
+    return LWB_E_UNSUPPORTED;
 }
 
 int launch(const Launch& L, cudaStream_t st)
 {
-    switch (L.n_tile) {
-        case 16:  return launch_one<16>(L, st);
-        case 32:  return launch_one<32>(L, st);
-        case 64:  return launch_one<64>(L, st);
-        case 128: return launch_one<128>(L, st);
-    }
-    lwb::set_error("conv_tc: unsupported N tile %d", L.n_tile);
-    return LWB_E_UNSUPPORTED;
+    return with_instance(L.n_tile, L.mode,
+                         [&](auto nt, auto md) { return launch_wg<decltype(nt)::value, decltype(md)::value>(L, st); });
 }
 
 int pick_n_tile(int cout, int forced)
@@ -656,6 +663,35 @@ int pick_n_tile(int cout, int forced)
     return -1;
 }
 
+// One tensor of a plan as a hi / lo pair of fp16 TMA views with the same shape.  dims innermost first, strides in bytes
+// for dims 1..rank-1; activations are rank 4 [C, W, H, N], weights rank 3 [K, N, tap].
+struct View {
+    const uint16_t* hi;
+    const uint16_t* lo;
+    uint64_t dims[4], str[3];
+};
+
+// What sets one launch of a plan apart; build_launch turns it into a Launch.
+struct LaunchSpec {
+    int ntaps;
+    signed char dy[MAX_TAPS], dx[MAX_TAPS], tmap[MAX_TAPS];
+    short wtap[MAX_TAPS];
+    int chunks0, chunks1;
+    int nviews;
+    View a[4];                          // activation views, indexed by tmap
+    View w;
+    int ncols;                          // GEMM N: cout, or 4 x cout for the merged transposed conv
+    int dom_h, dom_w;
+    int oy_mul, oy_add, ox_mul, ox_add, phase_cols;
+    int n_tile;
+
+    void tap(int y, int x, int view, int wt)
+    {
+        dy[ntaps] = (signed char)y; dx[ntaps] = (signed char)x; tmap[ntaps] = (signed char)view; wtap[ntaps] = (short)wt;
+        ntaps++;
+    }
+};
+
 }  // namespace
 
 struct lwb_conv_plan {
@@ -663,21 +699,27 @@ struct lwb_conv_plan {
     Launch launches[4];
 };
 
-// Plain NHWC activation map: dims [C, W, H, N], boxes of `rows` image rows.
-static int map_nhwc(CUtensorMap* m, const uint16_t* base, int n, int h, int w, int c, int rows)
+// NHWC activation view of every step-th pixel from (py, px): element (y', x') = input (step y' + py, step x' + px).
+// step 1 is the plain view, step 2 the parity views of stride-2 convs.
+static View nhwc_view(const uint16_t* hi, const uint16_t* lo, int n, int h, int w, int c, int step = 1, int py = 0, int px = 0)
 {
-    const uint64_t dims[4] = {(uint64_t)c, (uint64_t)w, (uint64_t)h, (uint64_t)n};
-    const uint64_t str[3] = {(uint64_t)c * 2, (uint64_t)w * c * 2, (uint64_t)h * w * c * 2};
-    const uint32_t box[4] = {(uint32_t)KCHUNK, TILE_W, (uint32_t)rows, 1};
-    return encode_map(m, base, 4, dims, str, box);
+    const size_t off = ((size_t)py * w + px) * c;
+    return View{hi + off, lo ? lo + off : lo,
+                {(uint64_t)c, (uint64_t)((w - px + step - 1) / step), (uint64_t)((h - py + step - 1) / step), (uint64_t)n},
+                {(uint64_t)step * c * 2, (uint64_t)step * w * c * 2, (uint64_t)h * w * c * 2}};
 }
-// Parity view (py, px) of an NHWC tensor for stride-2 convs: element (y', x') = input (2y'+py, 2x'+px).
-static int map_nhwc_parity(CUtensorMap* m, const uint16_t* base, int n, int h, int w, int c, int py, int px, int rows)
+
+// Weights [taps][ncols][k] fp16.
+static View weight_view(const uint16_t* hi, const uint16_t* lo, int k, int ncols, int taps)
 {
-    const uint64_t dims[4] = {(uint64_t)c, (uint64_t)((w - px + 1) / 2), (uint64_t)((h - py + 1) / 2), (uint64_t)n};
-    const uint64_t str[3] = {(uint64_t)2 * c * 2, (uint64_t)2 * w * c * 2, (uint64_t)h * w * c * 2};
-    const uint32_t box[4] = {(uint32_t)KCHUNK, TILE_W, (uint32_t)rows, 1};
-    return encode_map(m, base + ((size_t)py * w + px) * c, 4, dims, str, box);
+    return View{hi, lo, {(uint64_t)k, (uint64_t)ncols, (uint64_t)taps}, {(uint64_t)k * 2, (uint64_t)ncols * k * 2}};
+}
+
+// Encodes the hi map of a view, and in split mode its lo map.
+static int encode_pair(CUtensorMap* hi, CUtensorMap* lo, int rank, const View& v, const uint32_t* box, bool split)
+{
+    const int rc = encode_map(hi, v.hi, rank, v.dims, v.str, box);
+    return rc != LWB_OK || !split ? rc : encode_map(lo, v.lo, rank, v.dims, v.str, box);
 }
 
 // Orders the taps of p into y-halo groups: taps that read the same input view (tmap) at the same dx with consecutive
@@ -724,6 +766,36 @@ static void pick_rings(ConvParams& p, int n_tile, bool split)
     }
 }
 
+// The one path from a spec to a launch: y-halo groups, TMA maps, tile grid, ring depths and grid size.
+static int build_launch(Launch& L, const LaunchSpec& s, const lwb_conv_desc* d, float* out_raw, double* stats, int sms)
+{
+    const bool split = d->split != 0;
+    ConvParams& p = L.p;
+    memset(&p, 0, sizeof(p));
+    p.ntaps = s.ntaps; p.chunks0 = s.chunks0; p.chunks1 = s.chunks1;
+    for (int t = 0; t < s.ntaps; t++) { p.dy[t] = s.dy[t]; p.dx[t] = s.dx[t]; p.tmap[t] = s.tmap[t]; p.wtap[t] = s.wtap[t]; }
+    group_taps(p, tile_rows(s.n_tile));
+    int rc;
+    const uint32_t a_box[4] = {KCHUNK, TILE_W, (uint32_t)p.a_rows, 1};
+    for (int v = 0; v < s.nviews; v++)
+        if ((rc = encode_pair(&p.a_hi[v], &p.a_lo[v], 4, s.a[v], a_box, split)) != LWB_OK) return rc;
+    const uint32_t w_box[3] = {KCHUNK, (uint32_t)s.n_tile, 1};
+    if ((rc = encode_pair(&p.w_hi, &p.w_lo, 3, s.w, w_box, split)) != LWB_OK) return rc;
+    p.n_img = d->n;
+    p.dom_h = s.dom_h; p.dom_w = s.dom_w;
+    p.tiles_y = lwb::ceil_div(s.dom_h, tile_rows(s.n_tile)); p.tiles_x = lwb::ceil_div(s.dom_w, TILE_W);
+    p.n_tiles_n = s.ncols / s.n_tile;
+    p.out = out_raw; p.out_h = d->h_out; p.out_w = d->w_out; p.cout = d->cout;
+    p.oy_mul = s.oy_mul; p.oy_add = s.oy_add; p.ox_mul = s.ox_mul; p.ox_add = s.ox_add; p.phase_cols = s.phase_cols;
+    p.stats = stats;
+    p.out_scale = ldexpf(1.f, -d->w_exp);      // weights are packed x 2^w_exp in every operand mode (lwb_pack_conv_weight*)
+    L.n_tile = s.n_tile; L.mode = d->split;
+    pick_rings(p, s.n_tile, split);
+    const long total = (long)p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
+    L.grid = (int)(total < sms ? total : sms);
+    return LWB_OK;
+}
+
 extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
                                     const uint16_t* x0_hi, const uint16_t* x0_lo,
                                     const uint16_t* x1_hi, const uint16_t* x1_lo,
@@ -739,7 +811,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     LWB_CHECK_ARG(d->n > 0 && d->h_in > 0 && d->w_in > 0 && d->cout > 0, "non-positive size");
     LWB_CHECK_ARG(d->cout % 16 == 0, "cout must be a multiple of 16");
     LWB_CHECK_ARG(d->w_exp >= -40 && d->w_exp <= 60, "w_exp out of range");
-    int n_tile = pick_n_tile(d->cout, d->n_tile);
+    const int n_tile = pick_n_tile(d->cout, d->n_tile);
     LWB_CHECK_ARG(n_tile > 0 && d->cout % n_tile == 0, "no N tile divides cout");
     if (d->halo) {
         // halo plans ("same"-padded stride-1 k x k convs and the row-K stem) run through the tap-group kernel below
@@ -749,162 +821,93 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     }
 
     const int sms = lwb::sm_count();
-    lwb_conv_plan* plan = new (std::nothrow) lwb_conv_plan();
-    LWB_CHECK_ARG(plan, "out of host memory");
-    plan->num = 0;
-    int rc = LWB_OK;
-    auto fail = [&](int code) { delete plan; return code; };
 
-    auto finish = [&](Launch& L, int dom_h, int dom_w) {
-        ConvParams& p = L.p;
-        p.n_img = d->n;
-        p.dom_h = dom_h; p.dom_w = dom_w;
-        p.tiles_y = lwb::ceil_div(dom_h, tile_rows(n_tile)); p.tiles_x = lwb::ceil_div(dom_w, TILE_W);
-        p.n_tiles_n = d->cout / n_tile;
-        p.out = out_raw; p.out_h = d->h_out; p.out_w = d->w_out; p.cout = d->cout;
-        p.stats = stats;
-        p.out_scale = ldexpf(1.f, -d->w_exp);      // weights are packed x 2^w_exp in every operand mode (lwb_pack_conv_weight*)
-        L.n_tile = n_tile; L.mode = d->split;
-        pick_rings(p, n_tile, split);
-        const long total = (long)p.n_img * p.tiles_y * p.tiles_x * p.n_tiles_n;
-        L.grid = (int)(total < sms ? total : sms);
-    };
-
+    // Every variant starts from one stride-1 pass over the output grid with N = cout.
+    LaunchSpec s = {};
+    s.n_tile = n_tile; s.ncols = d->cout;
+    s.dom_h = d->h_out; s.dom_w = d->w_out;
+    s.oy_mul = s.ox_mul = 1;
+    s.nviews = 1;
+    LaunchSpec specs[4];
+    int num = 1;
     if (d->rowk) {
         // 7x7 stem through the row-K trick.  Input: padded NHWC8 buffer [n, h_in + kh - 1, wp, 8] whose
         // pixel (y + pad, x + pad) holds input pixel (y, x); wp >= w_in + 8.  One K = 64 stage = 8
         // consecutive pixels x 8 channels of a padded row = one whole filter row (8th tap weight = 0).
         LWB_CHECK_ARG(d->stride == 1 && !d->transposed && d->kw <= 8 && d->cin0 == 8 && d->cin1 == 0, "row-K needs stride 1, kw <= 8, 8 channels");
         LWB_CHECK_ARG(d->h_out == d->h_in && d->w_out == d->w_in && d->row_pitch >= d->w_in + 8, "row-K shape");
-        Launch& L = plan->launches[plan->num++];
-        memset(&L.p, 0, sizeof(L.p));
-        L.p.ntaps = d->kh; L.p.chunks0 = 1; L.p.chunks1 = 0;
-        for (int ky = 0; ky < d->kh; ky++) { L.p.dy[ky] = (signed char)ky; L.p.dx[ky] = 0; L.p.tmap[ky] = 0; L.p.wtap[ky] = (short)ky; }
-        group_taps(L.p, tile_rows(n_tile));
-        const int hp = d->h_in + d->kh - 1;
-        const uint64_t dims[4] = {64, (uint64_t)d->w_in, (uint64_t)hp, (uint64_t)d->n};
-        const uint64_t str[3] = {16, (uint64_t)d->row_pitch * 16, (uint64_t)hp * d->row_pitch * 16};
-        const uint32_t box[4] = {KCHUNK, TILE_W, (uint32_t)L.p.a_rows, 1};
-        if ((rc = encode_map(&L.p.a_hi[0], x0_hi, 4, dims, str, box)) != LWB_OK) return fail(rc);
-        if (split && (rc = encode_map(&L.p.a_lo[0], x0_lo, 4, dims, str, box)) != LWB_OK) return fail(rc);
-        const uint64_t wd[3] = {64, (uint64_t)d->cout, (uint64_t)d->kh};
-        const uint64_t ws[2] = {128, (uint64_t)d->cout * 128};
-        const uint32_t wb[3] = {KCHUNK, (uint32_t)n_tile, 1};
-        if ((rc = encode_map(&L.p.w_hi, w_hi, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
-        if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
-        L.p.oy_mul = 1; L.p.ox_mul = 1; L.p.oy_add = 0; L.p.ox_add = 0;
-        finish(L, d->h_out, d->w_out);
-        *plan_out = plan;
-        return LWB_OK;
-    }
-
-    LWB_CHECK_ARG(d->cin0 % KCHUNK == 0 && d->cin1 % KCHUNK == 0 && d->cin0 > 0, "input channels must be multiples of 64");
-    LWB_CHECK_ARG(d->cin1 == 0 || (x1_hi && (!split || x1_lo)), "second input missing");
-    const int cin_total = d->cin0 + d->cin1;
-    const int ntaps_w = d->kh * d->kw;
-    LWB_CHECK_ARG(ntaps_w <= MAX_TAPS, "too many filter taps");
-    const uint64_t wd[3] = {(uint64_t)cin_total, (uint64_t)d->cout, (uint64_t)ntaps_w};
-    const uint64_t ws[2] = {(uint64_t)cin_total * 2, (uint64_t)d->cout * cin_total * 2};
-    const uint32_t wb[3] = {(uint32_t)KCHUNK, (uint32_t)n_tile, 1};
-
-    if (d->transposed == 2) {
-        // Merged transposed conv: ONE stride-1 pass over the input grid with the four taps (dy, dx) in {0,1}^2 and
-        // N = 4 x cout columns = the four sub-pixel phases (weights from the host in [tap][phase*cout + co][cin] layout,
-        // zero where a phase does not use a tap: 9 of 16 blocks are non-zero).  One launch, one read of every input tile.
-        LWB_CHECK_ARG(d->kh == 3 && d->kw == 3 && d->stride == 2 && d->pad == 1 && d->cin1 == 0, "transposed conv: only k3 s2 p1 op1");
-        LWB_CHECK_ARG(d->h_out == 2 * d->h_in && d->w_out == 2 * d->w_in, "transposed conv output must be 2x input");
-        const int ncols = 4 * d->cout;
-        n_tile = MAX_N_TILE;                                  // the swapped N = 64 epilogue has no phase columns
-        LWB_CHECK_ARG(d->cout % 32 == 0 && ncols % n_tile == 0, "merged transposed conv needs cout in multiples of 32");
-        Launch& L = plan->launches[plan->num++];
-        memset(&L.p, 0, sizeof(L.p));
-        for (int t = 0; t < 4; t++) { L.p.dy[t] = (signed char)(t >> 1); L.p.dx[t] = (signed char)(t & 1); L.p.tmap[t] = 0; L.p.wtap[t] = (short)t; }
-        L.p.ntaps = 4; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = 0;
-        group_taps(L.p, tile_rows(n_tile));
-        if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
-        if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
-        const uint64_t mwd[3] = {(uint64_t)cin_total, (uint64_t)ncols, 4};
-        const uint64_t mws[2] = {(uint64_t)cin_total * 2, (uint64_t)ncols * cin_total * 2};
-        const uint32_t mwb[3] = {(uint32_t)KCHUNK, (uint32_t)n_tile, 1};
-        if ((rc = encode_map(&L.p.w_hi, w_hi, 3, mwd, mws, mwb)) != LWB_OK) return fail(rc);
-        if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, mwd, mws, mwb)) != LWB_OK) return fail(rc);
-        L.p.oy_mul = 2; L.p.ox_mul = 2; L.p.oy_add = 0; L.p.ox_add = 0;
-        finish(L, d->h_in, d->w_in);
-        L.p.phase_cols = d->cout;
-        L.p.n_tiles_n = ncols / n_tile;
-        const long total = (long)L.p.n_img * L.p.tiles_y * L.p.tiles_x * L.p.n_tiles_n;
-        L.grid = (int)(total < sms ? total : sms);
-        *plan_out = plan;
-        return LWB_OK;
-    }
-
-    if (d->transposed) {
-        // ConvTranspose2d(k=3, s=2, p=1, output_padding=1): out[2i+a, 2j+b] gathers, per axis,
-        //   a = 0: (k=1, d=0)            a = 1: (k=2, d=0), (k=0, d=+1)        (oy = 2*iy - 1 + ky)
-        LWB_CHECK_ARG(d->kh == 3 && d->kw == 3 && d->stride == 2 && d->pad == 1 && d->cin1 == 0, "transposed conv: only k3 s2 p1 op1");
-        LWB_CHECK_ARG(d->h_out == 2 * d->h_in && d->w_out == 2 * d->w_in, "transposed conv output must be 2x input");
-        for (int a = 0; a < 2; a++) for (int b = 0; b < 2; b++) {
-            Launch& L = plan->launches[plan->num++];
-            memset(&L.p, 0, sizeof(L.p));
-            const int ky_list[2][2] = {{1, -1}, {2, 0}}, d_list[2][2] = {{0, 0}, {0, 1}}, cnt[2] = {1, 2};
-            int t = 0;
-            for (int i = 0; i < cnt[a]; i++) for (int j = 0; j < cnt[b]; j++) {
-                L.p.dy[t] = (signed char)d_list[a][i]; L.p.dx[t] = (signed char)d_list[b][j];
-                L.p.tmap[t] = 0; L.p.wtap[t] = (short)(ky_list[a][i] * 3 + ky_list[b][j]);
-                t++;
-            }
-            L.p.ntaps = t; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = 0;
-            group_taps(L.p, tile_rows(n_tile));
-            if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
-            if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0, L.p.a_rows)) != LWB_OK) return fail(rc);
-            if ((rc = encode_map(&L.p.w_hi, w_hi, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
-            if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
-            L.p.oy_mul = 2; L.p.ox_mul = 2; L.p.oy_add = a; L.p.ox_add = b;
-            finish(L, d->h_in, d->w_in);
-        }
-        *plan_out = plan;
-        return LWB_OK;
-    }
-
-    LWB_CHECK_ARG(d->stride == 1 || d->stride == 2, "stride must be 1 or 2");
-    LWB_CHECK_ARG(d->stride == 1 || d->cin1 == 0, "concat input only with stride 1");
-    Launch& L = plan->launches[plan->num++];
-    memset(&L.p, 0, sizeof(L.p));
-    int t = 0;
-    for (int ky = 0; ky < d->kh; ky++) for (int kx = 0; kx < d->kw; kx++) {
-        const int oy = ky * d->dil - d->pad, ox = kx * d->dil - (d->pad_w >= 0 ? d->pad_w : d->pad);   // input offset relative to stride*y
-        if (oy < -127 || oy > 127 || ox < -127 || ox > 127) { lwb::set_error("conv_tc: tap offset out of range"); return fail(LWB_E_UNSUPPORTED); }
-        if (d->stride == 1) {
-            L.p.dy[t] = (signed char)oy; L.p.dx[t] = (signed char)ox; L.p.tmap[t] = 0;
-        } else {
-            // input coordinate 2y + oy = 2(y + floor(oy/2)) + (oy mod 2): parity view + index shift
-            const int py = ((oy % 2) + 2) % 2, px = ((ox % 2) + 2) % 2;
-            L.p.dy[t] = (signed char)((oy - py) / 2); L.p.dx[t] = (signed char)((ox - px) / 2);
-            L.p.tmap[t] = (signed char)(py * 2 + px);
-        }
-        L.p.wtap[t] = (short)t;
-        t++;
-    }
-    L.p.ntaps = t; L.p.chunks0 = d->cin0 / KCHUNK; L.p.chunks1 = d->cin1 / KCHUNK;
-    L.p.oy_mul = 1; L.p.ox_mul = 1; L.p.oy_add = 0; L.p.ox_add = 0;
-    group_taps(L.p, tile_rows(n_tile));
-    const int rows = L.p.a_rows;
-    if (d->stride == 1) {
-        if ((rc = map_nhwc(&L.p.a_hi[0], x0_hi, d->n, d->h_in, d->w_in, d->cin0, rows)) != LWB_OK) return fail(rc);
-        if (split && (rc = map_nhwc(&L.p.a_lo[0], x0_lo, d->n, d->h_in, d->w_in, d->cin0, rows)) != LWB_OK) return fail(rc);
-        if (d->cin1) {
-            if ((rc = map_nhwc(&L.p.a_hi[1], x1_hi, d->n, d->h_in, d->w_in, d->cin1, rows)) != LWB_OK) return fail(rc);
-            if (split && (rc = map_nhwc(&L.p.a_lo[1], x1_lo, d->n, d->h_in, d->w_in, d->cin1, rows)) != LWB_OK) return fail(rc);
-        }
+        for (int ky = 0; ky < d->kh; ky++) s.tap(ky, 0, 0, ky);
+        s.chunks0 = 1;
+        const uint64_t hp = d->h_in + d->kh - 1, row_bytes = (uint64_t)d->row_pitch * 16;
+        s.a[0] = View{x0_hi, x0_lo, {64, (uint64_t)d->w_in, hp, (uint64_t)d->n}, {16, row_bytes, hp * row_bytes}};
+        s.w = weight_view(w_hi, w_lo, 64, d->cout, d->kh);
     } else {
-        for (int py = 0; py < 2; py++) for (int px = 0; px < 2; px++) {
-            if ((rc = map_nhwc_parity(&L.p.a_hi[py * 2 + px], x0_hi, d->n, d->h_in, d->w_in, d->cin0, py, px, rows)) != LWB_OK) return fail(rc);
-            if (split && (rc = map_nhwc_parity(&L.p.a_lo[py * 2 + px], x0_lo, d->n, d->h_in, d->w_in, d->cin0, py, px, rows)) != LWB_OK) return fail(rc);
+        LWB_CHECK_ARG(d->cin0 % KCHUNK == 0 && d->cin1 % KCHUNK == 0 && d->cin0 > 0, "input channels must be multiples of 64");
+        LWB_CHECK_ARG(d->cin1 == 0 || (x1_hi && (!split || x1_lo)), "second input missing");
+        const int cin_total = d->cin0 + d->cin1;
+        const int ntaps_w = d->kh * d->kw;
+        LWB_CHECK_ARG(ntaps_w <= MAX_TAPS, "too many filter taps");
+        s.chunks0 = d->cin0 / KCHUNK; s.chunks1 = d->cin1 / KCHUNK;
+        s.a[0] = nhwc_view(x0_hi, x0_lo, d->n, d->h_in, d->w_in, d->cin0);
+        s.w = weight_view(w_hi, w_lo, cin_total, d->cout, ntaps_w);
+        if (d->transposed) {
+            // both transposed forms tile the input grid and write output pixel (2y + a, 2x + b)
+            LWB_CHECK_ARG(d->kh == 3 && d->kw == 3 && d->stride == 2 && d->pad == 1 && d->cin1 == 0, "transposed conv: only k3 s2 p1 op1");
+            LWB_CHECK_ARG(d->h_out == 2 * d->h_in && d->w_out == 2 * d->w_in, "transposed conv output must be 2x input");
+            s.dom_h = d->h_in; s.dom_w = d->w_in;
+            s.oy_mul = s.ox_mul = 2;
+        }
+        if (d->transposed == 2) {
+            // Merged transposed conv: ONE stride-1 pass over the input grid with the four taps (dy, dx) in {0,1}^2 and
+            // N = 4 x cout columns = the four sub-pixel phases (weights from the host in [tap][phase*cout + co][cin] layout,
+            // zero where a phase does not use a tap: 9 of 16 blocks are non-zero).  One launch, one read of every input tile.
+            s.n_tile = MAX_N_TILE;                            // the swapped N = 64 epilogue has no phase columns
+            s.ncols = 4 * d->cout;
+            LWB_CHECK_ARG(d->cout % 32 == 0 && s.ncols % s.n_tile == 0, "merged transposed conv needs cout in multiples of 32");
+            for (int t = 0; t < 4; t++) s.tap(t >> 1, t & 1, 0, t);
+            s.w = weight_view(w_hi, w_lo, cin_total, s.ncols, 4);
+            s.phase_cols = d->cout;
+        } else if (d->transposed) {
+            // ConvTranspose2d(k=3, s=2, p=1, output_padding=1): out[2i+a, 2j+b] gathers, per axis,
+            //   a = 0: (k=1, d=0)            a = 1: (k=2, d=0), (k=0, d=+1)        (oy = 2*iy - 1 + ky)
+            // one launch per sub-pixel phase (a, b)
+            const int ky_list[2][2] = {{1, -1}, {2, 0}}, d_list[2][2] = {{0, 0}, {0, 1}}, cnt[2] = {1, 2};
+            num = 4;
+            for (int a = 0; a < 2; a++) for (int b = 0; b < 2; b++) {
+                LaunchSpec& q = specs[a * 2 + b];
+                q = s;
+                for (int i = 0; i < cnt[a]; i++) for (int j = 0; j < cnt[b]; j++)
+                    q.tap(d_list[a][i], d_list[b][j], 0, ky_list[a][i] * 3 + ky_list[b][j]);
+                q.oy_add = a; q.ox_add = b;
+            }
+        } else {
+            LWB_CHECK_ARG(d->stride == 1 || d->stride == 2, "stride must be 1 or 2");
+            LWB_CHECK_ARG(d->stride == 1 || d->cin1 == 0, "concat input only with stride 1");
+            const int st = d->stride;
+            for (int ky = 0; ky < d->kh; ky++) for (int kx = 0; kx < d->kw; kx++) {
+                const int oy = ky * d->dil - d->pad, ox = kx * d->dil - (d->pad_w >= 0 ? d->pad_w : d->pad);   // input offset relative to stride*y
+                if (oy < -127 || oy > 127 || ox < -127 || ox > 127) { lwb::set_error("conv_tc: tap offset out of range"); return LWB_E_UNSUPPORTED; }
+                // input coordinate st y + oy = st (y + floor(oy / st)) + (oy mod st): view (py, px) + index shift
+                const int py = ((oy % st) + st) % st, px = ((ox % st) + st) % st;
+                s.tap((oy - py) / st, (ox - px) / st, py * 2 + px, s.ntaps);
+            }
+            // stride 2 reads four parity views of the input, a concat input (stride 1 only) a second tensor
+            s.nviews = st * st;
+            for (int v = 0; v < s.nviews; v++) s.a[v] = nhwc_view(x0_hi, x0_lo, d->n, d->h_in, d->w_in, d->cin0, st, v >> 1, v & 1);
+            if (d->cin1) {
+                s.nviews = 2;
+                s.a[1] = nhwc_view(x1_hi, x1_lo, d->n, d->h_in, d->w_in, d->cin1);
+            }
         }
     }
-    if ((rc = encode_map(&L.p.w_hi, w_hi, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
-    if (split && (rc = encode_map(&L.p.w_lo, w_lo, 3, wd, ws, wb)) != LWB_OK) return fail(rc);
-    finish(L, d->h_out, d->w_out);
+    if (num == 1) specs[0] = s;
+
+    lwb_conv_plan* plan = new (std::nothrow) lwb_conv_plan();
+    LWB_CHECK_ARG(plan, "out of host memory");
+    for (; plan->num < num; plan->num++) {
+        const int rc = build_launch(plan->launches[plan->num], specs[plan->num], d, out_raw, stats, sms);
+        if (rc != LWB_OK) { delete plan; return rc; }
+    }
     *plan_out = plan;
     return LWB_OK;
 }
@@ -957,20 +960,6 @@ extern "C" int lwb_conv_kernel_resources(int n_tile, int mode, int* out)
 {
     LWB_CHECK_ARG(out, "null pointer");
     LWB_CHECK_ARG(mode >= 0 && mode <= 2, "mode must be 0, 1 or 2");
-    switch (n_tile * 4 + mode) {
-        case 16 * 4 + 0:  return conv_resources<16, 0>(out);
-        case 16 * 4 + 1:  return conv_resources<16, 1>(out);
-        case 16 * 4 + 2:  return conv_resources<16, 2>(out);
-        case 32 * 4 + 0:  return conv_resources<32, 0>(out);
-        case 32 * 4 + 1:  return conv_resources<32, 1>(out);
-        case 32 * 4 + 2:  return conv_resources<32, 2>(out);
-        case 64 * 4 + 0:  return conv_resources<64, 0>(out);
-        case 64 * 4 + 1:  return conv_resources<64, 1>(out);
-        case 64 * 4 + 2:  return conv_resources<64, 2>(out);
-        case 128 * 4 + 0: return conv_resources<128, 0>(out);
-        case 128 * 4 + 1: return conv_resources<128, 1>(out);
-        case 128 * 4 + 2: return conv_resources<128, 2>(out);
-    }
-    lwb::set_error("conv_tc: unsupported N tile %d", n_tile);
-    return LWB_E_UNSUPPORTED;
+    return with_instance(n_tile, mode,
+                         [&](auto nt, auto md) { return conv_resources<decltype(nt)::value, decltype(md)::value>(out); });
 }
