@@ -167,9 +167,10 @@ extern "C" int lwb_conv2d_direct_nchw(const float* x, const float* w, const floa
 {
     LWB_CHECK_ARG(x && w && out, "null pointer");
     LWB_CHECK_ARG(n > 0 && cin > 0 && h > 0 && wd > 0 && cout > 0 && kh > 0 && kw > 0 && stride > 0 && dil > 0 && pad >= 0, "bad sizes");
+    // the dilated filter must fit the padded input: below that, C's truncating division would still give one row
+    LWB_CHECK_ARG(h + 2 * pad >= dil * (kh - 1) + 1 && wd + 2 * pad >= dil * (kw - 1) + 1 && n <= 65535, "empty output");
     const int ho = (h + 2 * pad - dil * (kh - 1) - 1) / stride + 1;
     const int wo = (wd + 2 * pad - dil * (kw - 1) - 1) / stride + 1;
-    LWB_CHECK_ARG(ho > 0 && wo > 0 && n <= 65535, "empty output");
     dim3 grid(lwb::ceil_div((long)ho * wo, 256), lwb::ceil_div(cout, 4), n);
     k_conv_direct<false><<<grid, 256, 0, (cudaStream_t)stream>>>(x, w, bias, cin, h, wd, cout, kh, kw, stride, pad, dil, ho, wo, out);
     LWB_LAUNCH_OK();

@@ -418,8 +418,8 @@ __global__ void __launch_bounds__(256) k_heads(const float* __restrict__ raw, in
     if (range_flag) {
         // Output-head pre-activations of +-8 and more: the ~1e-4 end-to-end RELATIVE precision of the fp16f8 operand split is
         // then no longer enough for 1e-3 on the (unsaturated) pixels -- report it (bit 2), the caller switches to fp16x3.
-        const float m = fmaxf(fmaxf(fabsf(r.x), fabsf(r.y)), fmaxf(fabsf(r.z), fabsf(r.w)));
-        const bool big = !(m < 8.f);
+        // (fmaxf would drop a NaN component, so each one is compared on its own)
+        const bool big = !(fabsf(r.x) < 8.f && fabsf(r.y) < 8.f && fabsf(r.z) < 8.f && fabsf(r.w) < 8.f);
         if (__any_sync(__activemask(), big) && big && !(*reinterpret_cast<volatile int*>(range_flag) & 4)) atomicOr(range_flag, 4);
     }
     const float col[3] = {tanhf(r.x), tanhf(r.y), tanhf(r.z)};

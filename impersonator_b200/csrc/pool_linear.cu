@@ -7,7 +7,7 @@
 namespace {
 
 // F.max_pool2d(x, kernel_size=k, stride=s, ceil_mode=True), no padding (networks/hmr.py:150):
-// out = ceil((in - k) / s) + 1 windows, the last one clipped at the border.  NCHW in -> NHWC out.
+// out = ceil_pool_out(in, k, s) windows, the last one clipped at the border.  NCHW in -> NHWC out.
 __global__ void __launch_bounds__(256) k_maxpool_nchw_to_nhwc(const float* __restrict__ x, int n, int c, int h, int w,
                                                               int k, int s, int ho, int wo, float* __restrict__ out)
 {
@@ -101,13 +101,21 @@ __global__ void __launch_bounds__(256) k_linear(const float* __restrict__ x, int
     }
 }
 
+// torch's ceil-mode output size without padding: ceil((in - k) / s) + 1, less a last window that would start at or past
+// the end of the input (possible when k < s)
+int ceil_pool_out(int in, int k, int s)
+{
+    const int o = lwb::ceil_div(in - k, s) + 1;
+    return (o - 1) * s >= in ? o - 1 : o;
+}
+
 }  // namespace
 
 extern "C" int lwb_maxpool_nchw_to_nhwc(const float* x, int n, int c, int h, int w, int k, int stride, float* out, lwb_stream_t stream)
 {
     LWB_CHECK_ARG(x && out, "null pointer");
     LWB_CHECK_ARG(n > 0 && c > 0 && h >= k && w >= k && k > 0 && stride > 0, "bad sizes");
-    const int ho = lwb::ceil_div(h - k, stride) + 1, wo = lwb::ceil_div(w - k, stride) + 1;
+    const int ho = ceil_pool_out(h, k, stride), wo = ceil_pool_out(w, k, stride);
     const long total = (long)n * ho * wo * c;
     k_maxpool_nchw_to_nhwc<<<lwb::ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(x, n, c, h, w, k, stride, ho, wo, out);
     LWB_LAUNCH_OK();

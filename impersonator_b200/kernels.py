@@ -500,11 +500,17 @@ def self_attention_nhwc(qkv, bias, x, gamma, dq=16, out=None):
     return out
 
 
+def _ceil_pool_out(size, k, stride):
+    """torch's ceil_mode output size without padding: a last window that would start past the input is dropped."""
+    o = -(-(size - k) // stride) + 1
+    return o - 1 if (o - 1) * stride >= size else o
+
+
 def maxpool_nchw_to_nhwc(x, k, stride, out=None):
     """F.max_pool2d(x, k, stride, ceil_mode=True) (networks/hmr.py:150): NCHW fp32 -> NHWC fp32."""
     _chk_cuda(x, out)
     n, c, h, w = x.shape
-    ho, wo = -(-(h - k) // stride) + 1, -(-(w - k) // stride) + 1
+    ho, wo = _ceil_pool_out(h, k, stride), _ceil_pool_out(w, k, stride)
     if out is None:
         out = torch.empty((n, ho, wo, c), dtype=torch.float32, device=x.device)
     _count(1)

@@ -1,0 +1,669 @@
+"""Seeded cases of the glue kernels around the conv engine, shared by test_glue_kernels_gpu.py (the CUDA front-ends of
+impersonator_b200.kernels) and test_glue_cases_cpu.py (their torch stand-ins in kernel_emulator).
+
+A case is one call of one front-end on CPU-built inputs.  ``run(api, put, alloc)`` makes the call through ``api`` (the
+kernels module or the emulator); ``put`` moves an input to the device, ``alloc`` turns a CPU tensor into the caller buffer
+the front-end writes (a sentinel-guarded view on the GPU).  The checks compare the outputs with a float64 restatement of
+the operation from torch / numpy, never with the emulator:
+
+* ``Bits``: exact contracts (layout moves, max, fp16 operand splits, uint8 truncation, range-flag bits);
+* ``Tol``: |got - ref| <= tau * 2^-24 * S per element, S = the sum of |terms| (the same restatement on |inputs|) or, for
+  elementwise operations, the magnitude the rounding scales with.  Each Tol also asserts tol < 0.1 * S / K for its K
+  terms, so no bar is wide enough to hide a dropped, duplicated or shifted term.
+
+Every required edge below names one case; the CPU suite checks that each front-end the emulator replaces has all its
+edges, or an entry in COVERED_ELSEWHERE naming the test that covers it.
+"""
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+U32 = 2.0 ** -24               # fp32 unit roundoff
+TAU = 16
+NAN = float("nan")
+
+
+# ------------------------------------------------------------------------------------------------------------ checks
+def _get(outs, out):
+    return out(outs) if callable(out) else outs[out]
+
+
+class Tol(object):
+    def __init__(self, label, out, ref, S, K, tau=TAU, unit=U32, kernel_only=False):
+        self.label, self.out, self.ref, self.S, self.K = label, out, ref.double(), S.double(), K
+        self.tau, self.unit, self.kernel_only = tau, unit, kernel_only
+
+    def __call__(self, case, outs):
+        got = _get(outs, self.out).double()
+        assert got.shape == self.ref.shape, "%s/%s: shape %s, want %s" % (case, self.label, tuple(got.shape), tuple(self.ref.shape))
+        tol = self.tau * self.unit * self.S
+        pos = self.S > 0
+        assert bool((tol[pos] < 0.1 * self.S[pos] / self.K).all()), \
+            "%s/%s: tol %g * S is not below a tenth of one of the %d terms" % (case, self.label, self.tau * self.unit, self.K)
+        err = (got - self.ref).abs()
+        ratio = torch.where(tol > 0, err / tol.clamp(min=1e-300), torch.where(err > 0, float("inf"), 0.0))
+        ratio = torch.where(torch.isnan(err), float("inf"), ratio)
+        r = float(ratio.max()) if ratio.numel() else 0.0
+        print("%s/%s: max err %.3g, max err/tol %.3f (K=%d)" % (case, self.label, float(err.max()) if err.numel() else 0.0, r, self.K))
+        assert r <= 1.0, "%s/%s: error %.3g times the bar at %s" % (case, self.label, r, tuple(int(i) for i in np.unravel_index(
+            int(ratio.flatten().argmax()), tuple(ratio.shape))))
+
+
+class Bits(object):
+    """Byte-identical to ``want`` (a tensor, or a function of the outputs for contracts stated on the kernel's own
+    results)."""
+
+    def __init__(self, label, out, want, kernel_only=False):
+        self.label, self.out, self.want, self.kernel_only = label, out, want, kernel_only
+
+    def __call__(self, case, outs):
+        got = _get(outs, self.out).contiguous()
+        want = (self.want(outs) if callable(self.want) else self.want).contiguous()
+        assert got.dtype == want.dtype and got.shape == want.shape, "%s/%s: %s %s, want %s %s" % (
+            case, self.label, got.dtype, tuple(got.shape), want.dtype, tuple(want.shape))
+        g, w = got.view(torch.uint8), want.view(torch.uint8)
+        bad = (g != w).nonzero()
+        print("%s/%s: %d of %d bytes differ" % (case, self.label, bad.shape[0], g.numel()))
+        assert bad.shape[0] == 0, "%s/%s: first difference at byte %s (got %d, want %d)" % (
+            case, self.label, tuple(bad[0].tolist()), int(g[tuple(bad[0])]), int(w[tuple(bad[0])]))
+
+
+def Flag(want):
+    return Bits("range_flag", "flag", torch.tensor([want], dtype=torch.int32))
+
+
+class Case(object):
+    def __init__(self, front, edge, run, checks, emulated=True):
+        self.front, self.edge, self.run, self.checks, self.emulated = front, edge, run, checks, emulated
+        self.name = "%s/%s" % (front, edge)
+
+
+# ---------------------------------------------------------------------------------------------------------- helpers
+def _gen(seed):
+    return torch.Generator().manual_seed(seed)
+
+
+def _randn(g, *shape, scale=1.0, shift=0.0):
+    return torch.randn(*shape, generator=g) * scale + shift
+
+
+def _full(shape, value=NAN, dtype=torch.float32):
+    return torch.full(shape, value, dtype=dtype)
+
+
+def _put_all(put, *ts):
+    return [put(t) if t is not None else None for t in ts]
+
+
+def _nchw(t):
+    return t.permute(0, 3, 1, 2)
+
+
+def _nhwc(t):
+    return t.permute(0, 2, 3, 1)
+
+
+def fp16_pair(v):
+    hi = v.half()
+    return hi, (v - hi.float()).half()
+
+
+def u8_bgr(hwc):
+    """cv_utils.save_cv2_img's ((img + 1) / 2.0 * 255).astype(np.uint8) in float32 numpy, channels reversed (RGB2BGR)."""
+    a = hwc.numpy().astype(np.float32)
+    return torch.from_numpy(((a + 1) / 2.0 * 255).astype(np.uint8)[..., ::-1].copy())
+
+
+def _flow(g, n, th, tw):
+    """Flow in [-1.1, 1.1] with about 15% of the pixels at -2 (the background code of the correspondence maps)."""
+    T = torch.rand(n, th, tw, 2, generator=g) * 2.2 - 1.1
+    bgm = torch.rand(n, th, tw, 1, generator=g) < 0.15
+    return torch.where(bgm, torch.full_like(T, -2.0), T)
+
+
+def _warp64(src_nchw, T, h, w, ac, n):
+    """grid_sample(src, resize(T)) in float64 and its S: the bilinear terms on |src|, plus the tap weights' sensitivity
+    to the fp32 rounding of the sample coordinate (about 2^-24 (h + w) pixels per tap, flow magnitudes up to 2)."""
+    src = src_nchw.double().expand(n, -1, -1, -1)
+    Ts = T.double()
+    if tuple(Ts.shape[1:3]) != (h, w):
+        Ts = _nhwc(F.interpolate(_nchw(Ts), size=(h, w), mode="bilinear", align_corners=True))
+    val = F.grid_sample(src, Ts, mode="bilinear", padding_mode="zeros", align_corners=bool(ac))
+    mag = F.grid_sample(src.abs(), Ts, mode="bilinear", padding_mode="zeros", align_corners=bool(ac))
+    return val, mag + 8 * (h + w) * src.abs().amax(dim=(2, 3), keepdim=True)
+
+
+# --------------------------------------------------------------------------------------------------------- norm_act
+def _norm_act(edge, seed, n, h, w, c, mode="stats", relu=False, res_step=0, warp=None, post=None, lo_format=0, raw=None,
+              flag=None):
+    """mode: stats (InstanceNorm, gamma and beta) | affine (gamma, beta) | affine_g | affine_b | bare;
+    warp: (src_batch, th, tw, align_corners); post: post_relu (bool) for the EXT variant's second affine."""
+    g = _gen(seed)
+    if raw is None:
+        raw = _randn(g, n, h, w, c, scale=2.0, shift=0.5)
+        if mode == "stats":                 # channel 0: mean 4e4 x its std (the fused x * scale + shift keeps ~1e-3)
+            raw[..., 0] = _randn(g, n, h, w, shift=4e4)
+    gamma = _randn(g, c, scale=0.1, shift=1.0) if mode in ("stats", "affine", "affine_g") else None
+    beta = _randn(g, c, scale=0.1) if mode in ("stats", "affine", "affine_b") else None
+    res = _randn(g, n, h * res_step, w * res_step, c) if res_step else None
+    src = T = None
+    if warp is not None:
+        sb, th, tw, ac = warp
+        src = _randn(g, sb, h, w, c)
+        T = _flow(g, n, th, tw)
+    ps = pt = None
+    if post is not None:
+        ps, pt = _randn(g, c, scale=0.2, shift=1.0), _randn(g, c, scale=0.3)
+
+    x = raw.double()
+    stats = None
+    if mode == "stats":
+        stats = torch.stack([x.sum(dim=(1, 2)), (x * x).sum(dim=(1, 2))], dim=-1)          # the conv epilogue's f64 sums
+        mean = x.mean(dim=(1, 2))
+        var = ((x - mean[:, None, None, :]) ** 2).mean(dim=(1, 2))
+        scale = gamma.double() / torch.sqrt(var + 1e-5)
+        shift = beta.double() - mean * scale
+        sc, sh = scale[:, None, None, :], shift[:, None, None, :]
+        y = x * sc + sh
+        S = (x * sc).abs() + (mean[:, None, None, :] * sc).abs() + beta.double().abs()
+    elif mode == "bare":
+        y, S = x.clone(), x.abs()
+    else:
+        gm = gamma.double() if gamma is not None else 1.0
+        bt = beta.double() if beta is not None else torch.zeros(c, dtype=torch.float64)
+        y, S = x * gm + bt, (x * gm).abs() + bt.abs()
+    K = 2
+    if relu:
+        y = y.clamp(min=0)
+    if res is not None:
+        r = res[:, ::res_step, ::res_step, :].double()
+        y, S, K = y + r, S + r.abs(), K + 1
+    if warp is not None:
+        wv, ws_ = _warp64(_nchw(src), T, h, w, warp[3], n)
+        y, S, K = y + _nhwc(wv), S + _nhwc(ws_), K + 4
+    norm = mode != "bare"
+
+    def run(api, put, alloc):
+        o = {"y_f32": alloc(_full((n, h, w, c)))}
+        o["hi"] = alloc(_full((n, h, w, c), dtype=torch.float16))
+        o["lo"] = alloc(_full((n, h, w, c), dtype=torch.float16))
+        if flag is not None:
+            o["flag"] = alloc(torch.zeros(1, dtype=torch.int32))
+        ws = alloc(torch.zeros(n, c, 2)) if norm else None
+        r_, st, ga, be, re, sr, Td, psd, ptd = _put_all(put, raw, stats, gamma, beta, res, src, T, ps, pt)
+        api.norm_act_nhwc(r_, st, ga, be, relu, ws, residual=re, warp_src=sr, T=Td,
+                          align_corners=bool(warp[3]) if warp else False, y_f32=o["y_f32"], y_hi=o["hi"], y_lo=o["lo"],
+                          lo_format=lo_format, post_scale=psd, post_shift=ptd, post_relu=bool(post),
+                          res_step=res_step or 1, range_flag=o.get("flag"))
+        return o
+
+    if flag is not None:                 # the range cases: y = raw, only the flag bits matter (hi of NaN is not pinned)
+        return Case("norm_act_nhwc", edge, run, [Bits("y_f32", "y_f32", raw), Flag(flag)])
+    checks = [Bits("y_f32", "y_f32", raw) if (mode == "bare" and warp is None) else Tol("y_f32", "y_f32", y, S, K)]
+    if post is None:
+        checks.append(Bits("hi", "hi", lambda o: fp16_pair(o["y_f32"])[0]))
+        if lo_format == 0:
+            checks.append(Bits("lo", "lo", lambda o: fp16_pair(o["y_f32"])[1]))
+        else:
+            def lo8(o):
+                from test_conv_emulation_gpu import pair_blocks
+                v = o["y_f32"]
+                return pair_blocks(v / 16, (v - v.half().float()) * 1024)
+            checks.append(Bits("lo8", lambda o: o["lo"].view(torch.uint8), lo8, kernel_only=True))
+    else:
+        z = y * ps.double() + pt.double()
+        if post:
+            z = z.clamp(min=0)
+        checks.append(Tol("hi+lo (post affine)", lambda o: o["hi"].double() + o["lo"].double(), z,
+                          S * ps.double().abs() + pt.double().abs(), K + 1))
+    return Case("norm_act_nhwc", edge, run, checks)
+
+
+def norm_act_cases():
+    cases = []
+    for c in (8, 16, 64, 128, 256, 512, 1024, 2048):            # groups 1 .. 256; 105 pixels: a partial last block
+        cases.append(_norm_act("stats c=%d" % c, 200 + c, 3, 7, 5, c, relu=True))
+    cases += [
+        _norm_act("affine gamma+beta", 301, 2, 5, 3, 64, mode="affine"),
+        _norm_act("affine gamma only", 302, 2, 5, 3, 64, mode="affine_g", relu=True),
+        _norm_act("affine beta only", 303, 2, 5, 3, 64, mode="affine_b"),                 # hmr.py: gamma=None, beta=bias
+        _norm_act("bare", 304, 2, 3, 7, 128, mode="bare"),
+        _norm_act("stats relu residual", 305, 2, 9, 4, 64, relu=True, res_step=1),
+        _norm_act("bare warp", 306, 2, 6, 10, 32, mode="bare", warp=(1, 16, 20, 1)),      # generator.py _add_warp
+        _norm_act("EXT post affine res_step 2", 307, 2, 5, 3, 64, mode="affine_b", res_step=2, post=True),
+        _norm_act("EXT res_step 2", 308, 2, 5, 3, 64, relu=True, res_step=2),
+        _norm_act("lo_format 1 c=512", 309, 1, 3, 5, 512, relu=True, lo_format=1),
+    ]
+    for sb in ("1", "n"):
+        for tsize in ("same", "larger"):
+            for ac in (0, 1):
+                n, h, w = 2, 6, 10
+                th, tw = (h, w) if tsize == "same" else (16, 20)
+                cases.append(_norm_act("warp sb=%s T %s ac=%d" % (sb, tsize, ac), 310 + 4 * (sb == "n") + 2 * (tsize == "same") + ac,
+                                       n, h, w, 32, relu=ac == 0, res_step=1 if sb == "n" else 0,
+                                       warp=(1 if sb == "1" else n, th, tw, ac)))
+    # fp16 of the emitted value: 1023.7 -> 1023.5, 1023.75 -> 1024 (tie to even), 59983 / 59984 -> 59968 (tie to even),
+    # 59990 -> 60000 = 0x7b53, 65520 -> inf
+    for label, v, want in (("1023.7", 1023.7, 0), ("1023.75", 1023.75, 1), ("1024", 1024.0, 1), ("-1024", -1024.0, 1),
+                           ("59984", 59984.0, 1), ("59990", 59990.0, 3), ("60000", 60000.0, 3), ("65520", 65520.0, 3),
+                           ("+inf", float("inf"), 3), ("-inf", float("-inf"), 3), ("nan", NAN, 3)):
+        raw = torch.rand(1, 3, 5, 8, generator=_gen(400)) * 8 - 4
+        raw[0, 1, 2, 5] = v
+        cases.append(_norm_act("range %s" % label, 400, 1, 3, 5, 8, mode="bare", raw=raw, flag=want))
+    return cases
+
+
+# --------------------------------------------------------------------------------------------------- instance_stats
+def _instance_stats(edge, seed, n, h, w, c):
+    x = _randn(_gen(seed), n, h, w, c, scale=3.0, shift=1.0)
+    xd = x.double()
+    ref = torch.stack([xd.sum(dim=(1, 2)), (xd * xd).sum(dim=(1, 2))], dim=-1)
+    S = torch.stack([xd.abs().sum(dim=(1, 2)), (xd * xd).sum(dim=(1, 2))], dim=-1)
+
+    def run(api, put, alloc):
+        st = alloc(torch.zeros(n, c, 2, dtype=torch.float64))
+        api.instance_stats_nhwc(put(x), st)
+        return {"stats": st}
+    # exact f64 sums of exact products: 8192 * 2^-53 ~ 1e-12 relative
+    return Case("instance_stats_nhwc", edge, run, [Tol("stats", "stats", ref, S, h * w, tau=8192, unit=2.0 ** -53)],
+                emulated=False)
+
+
+def instance_stats_cases():
+    return [_instance_stats("hw=35 c=40", 501, 2, 5, 7, 40),             # one split, hw % 8 != 0
+            _instance_stats("hw=1000 c=96", 502, 2, 20, 50, 96),          # three splits
+            _instance_stats("hw=16640 c=33", 503, 1, 128, 130, 33)]       # 64 splits, c % 32 != 0
+
+
+# --------------------------------------------------------------------------------------------- heads / frames out
+def _fold(raw, kw):
+    """out[y, x, co] = sum_kx raw[y, x + kx - kw/2, kx*4 + co] over the columns inside the image."""
+    if not kw:
+        return raw[..., :4]
+    w = raw.shape[2]
+    r = torch.zeros(raw.shape[:3] + (4,), dtype=raw.dtype)
+    for kx in range(kw):
+        sh = kx - kw // 2
+        x0, x1 = max(0, -sh), min(w, w - sh)
+        if x1 > x0:
+            r[:, :, x0:x1] += raw[:, :, x0 + sh:x1 + sh, kx * 4:kx * 4 + 4]
+    return r
+
+
+def sweep_values():
+    """Float32 values at and a few ulps around every boundary 2k/255 - 1 of the uint8 cast, and +-1 exactly."""
+    vals = [np.float32(-1.0), np.float32(1.0)]
+    for k in range(256):
+        b = np.float32(2.0 * k / 255.0 - 1.0)
+        v = b
+        for _ in range(4):
+            v = np.nextafter(v, np.float32(-2))
+            vals.append(v)
+        vals.append(b)
+        v = b
+        for _ in range(4):
+            v = np.nextafter(v, np.float32(2))
+            vals.append(v)
+    return torch.from_numpy(np.array(vals, dtype=np.float32))
+
+
+def _sweep_frames(h, w):
+    v = sweep_values()
+    flat = torch.full((3 * h * w,), 0.5)
+    flat[:v.numel()] = v
+    return flat.view(1, 3, h, w)
+
+
+def _heads(edge, seed, n, h, w, cs, kw, bg_batch, raw=None, bg=None, flag=0, flag_only=False):
+    g = _gen(seed)
+    if raw is None:
+        raw = torch.rand(n, h, w, cs, generator=g) * 2 - 1           # folded sums stay below 7: range bit 2 clear
+    if bg is None and not flag_only:
+        bg = torch.rand(bg_batch, 3, h, w, generator=g) * 2 - 1
+
+    def run(api, put, alloc):
+        o = {"color": alloc(_full((n, 3, h, w))), "mask": alloc(_full((n, 1, h, w))), "flag": alloc(torch.zeros(1, dtype=torch.int32))}
+        if bg is not None:
+            o["pred"] = alloc(_full((n, 3, h, w)))
+            o["pred_hwc"] = alloc(_full((n, h, w, 3)))
+            o["pred_u8"] = alloc(torch.full((n, h, w, 3), 77, dtype=torch.uint8))
+        api.heads_composite(put(raw), put(bg), color=o["color"], mask=o["mask"], pred=o.get("pred"), pred_hwc=o.get("pred_hwc"),
+                            pred_u8=o.get("pred_u8"), folded_kw=kw, range_flag=o["flag"])
+        return o
+
+    if flag_only:
+        return Case("heads_composite", edge, run, [Flag(flag)])
+    r, Sr = _fold(raw.double(), kw), _fold(raw.double().abs(), kw)
+    K = max(kw, 1)
+    col, m = torch.tanh(_nchw(r[..., :3])), torch.sigmoid(_nchw(r[..., 3:]))
+    Sc, Sm = _nchw(Sr[..., :3]), _nchw(Sr[..., 3:])
+    b = bg.double().expand(n, -1, -1, -1)
+    pred = m * b + (1 - m) * col
+    checks = [Tol("color (tanh)", "color", col, Sc + col.abs(), K),
+              Tol("mask (sigmoid)", "mask", m, Sm + m, K),
+              Tol("pred", "pred", pred, (b.abs() + col.abs() + 1) * (Sc + Sm + 1), 2),
+              Bits("pred_hwc", "pred_hwc", lambda o: _nhwc(o["pred"]).contiguous()),
+              Bits("pred_u8", "pred_u8", lambda o: u8_bgr(o["pred_hwc"])),
+              Flag(flag)]
+    return Case("heads_composite", edge, run, checks)
+
+
+def heads_cases():
+    cases = []
+    for w in (1, 2, 3, 70):                # w = 2: the folded columns reach past both borders of a pixel
+        for kw, cs, bgb in ((0, 4, "1"), (0, 32, "n"), (7, 32, "1"), (7, 32, "n")):
+            cases.append(_heads("kw=%d w=%d c_stride=%d bg_batch=%s" % (kw, w, cs, bgb), 600 + w + kw + cs, 2, 3, w, cs, kw,
+                                1 if bgb == "1" else 2))
+    # the composite is bg exactly where the mask saturates to 1 (|pre-activation| 20 also sets range bit 2)
+    h, w = 13, 60
+    raw = torch.rand(1, h, w, 4, generator=_gen(650)) * 2 - 1
+    raw[..., 3] = 20.0
+    cases.append(_heads("u8 sweep", 650, 1, h, w, 4, 0, 1, raw=raw, bg=_sweep_frames(h, w), flag=4))
+    for label, v, ch, want in (("8.0", 8.0, 0, 4), ("below 8.0", float(np.nextafter(np.float32(8), np.float32(0))), 1, 0),
+                               ("-8.0", -8.0, 3, 4), ("nan", NAN, 2, 4)):
+        raw = torch.rand(1, 2, 3, 4, generator=_gen(660)) * 2 - 1
+        raw[0, 1, 2, ch] = v
+        cases.append(_heads("range %s" % label, 660, 1, 2, 3, 4, 0, 1, raw=raw, flag=want, flag_only=True))
+    return cases
+
+
+def frames_out_cases():
+    frames = _sweep_frames(13, 60)
+
+    def run(api, put, alloc):
+        hwc, u8 = api.frames_out(put(frames), want_hwc=True, want_u8=True)
+        return {"hwc": hwc, "u8": u8}
+    return [Case("frames_out", "u8 sweep", run, [Bits("hwc", "hwc", _nhwc(frames).contiguous()),
+                                                 Bits("u8", "u8", u8_bgr(_nhwc(frames)))], emulated=False)]
+
+
+# ------------------------------------------------------------------------------------------------------ direct conv
+def _conv_direct(edge, seed, n, cin, h, w, cout, k, stride=1, pad=0, dil=1, bias=True):
+    g = _gen(seed)
+    x, wt = _randn(g, n, cin, h, w), _randn(g, cout, cin, k, k, scale=0.2)
+    b = _randn(g, cout) if bias else None
+    conv = lambda a, ww, bb: F.conv2d(a, ww, bb, stride=stride, padding=pad, dilation=dil)      # noqa: E731
+    ref = conv(x.double(), wt.double(), b.double() if bias else None)
+    S = conv(x.double().abs(), wt.double().abs(), b.double().abs() if bias else None)
+
+    def run(api, put, alloc):
+        return {"out": api.conv2d_direct_nchw(put(x), put(wt), put(b) if bias else None, stride=stride, pad=pad, dil=dil)}
+    return Case("conv2d_direct_nchw", edge, run, [Tol("out", "out", ref, S, cin * k * k + 1)])
+
+
+def conv_direct_cases():
+    return [_conv_direct("cout=7", 701, 2, 5, 9, 8, 7, 3, pad=1),
+            _conv_direct("dilation 2", 702, 1, 5, 12, 10, 4, 3, pad=2, dil=2),
+            _conv_direct("stride 2 odd sizes", 703, 2, 3, 9, 11, 5, 3, stride=2, pad=1),
+            _conv_direct("pad > k/2", 704, 1, 4, 6, 7, 4, 3, pad=3),
+            _conv_direct("bias None", 705, 2, 5, 8, 8, 6, 3, pad=1, bias=False),
+            _conv_direct("1x1", 706, 2, 6, 7, 5, 9, 1),
+            _conv_direct("inpaintor 5x5", 707, 1, 5, 20, 20, 8, 5, pad=2),
+            _conv_direct("inpaintor 4x4 s2", 708, 1, 8, 20, 20, 6, 4, stride=2, pad=1),
+            _conv_direct("inpaintor 3x3 dil 16", 709, 1, 6, 40, 36, 5, 3, pad=16, dil=16)]
+
+
+# --------------------------------------------------------------------------------------------------------- 7x7 heads
+def _heads7x7(edge, seed, n, h, w):
+    g = _gen(seed)
+    x = _randn(g, n, h, w, 64)
+    wi, wa = _randn(g, 3, 64, 7, 7, scale=0.02), _randn(g, 1, 64, 7, 7, scale=0.02)
+    wt = torch.cat([wi, wa]).double()
+    ref = _nhwc(F.conv2d(_nchw(x.double()), wt, padding=3))
+    S = _nhwc(F.conv2d(_nchw(x.double().abs()), wt.abs(), padding=3))
+
+    def run(api, put, alloc):
+        out = alloc(_full((n, h, w, 4)))
+        api.conv7x7_heads_nhwc(put(x), api.pack_head_weights(put(wi), put(wa)), out=out)
+        return {"out": out}
+    return Case("conv7x7_heads_nhwc", edge, run, [Tol("out", "out", ref, S, 64 * 49)])
+
+
+def heads7x7_cases():
+    return [_heads7x7("1x1", 801, 2, 1, 1), _heads7x7("5x3", 802, 2, 5, 3), _heads7x7("17x65", 803, 1, 17, 65)]
+
+
+# --------------------------------------------------------------------------------------------------------- gated BN
+def _gated_bn(act, with_scale, seed):
+    g = _gen(seed)
+    n, c, h, w = 2, 5, 3, 7
+    ab = _randn(g, n, 2 * c, h, w, scale=2.0)
+    sc, sh = (_randn(g, c, scale=0.3, shift=1.0), _randn(g, c, scale=0.5)) if with_scale else (None, None)
+    a, gt = ab[:, :c].double(), ab[:, c:].double()
+    a = F.leaky_relu(a, 0.2) if act == 2 else (a.clamp(min=0) if act == 1 else a)
+    y = a * torch.sigmoid(gt)
+    S = y.abs()
+    if with_scale:
+        y = y * sc.double()[None, :, None, None] + sh.double()[None, :, None, None]
+        S = S * sc.double().abs()[None, :, None, None] + sh.double().abs()[None, :, None, None]
+
+    def run(api, put, alloc):
+        return {"out": api.gated_bn_nchw(put(ab), act, put(sc) if with_scale else None, put(sh) if with_scale else None)}
+    # sigmoid through expf and a division, the product, the fused affine: a few ulps of S
+    return Case("gated_bn_nchw", "act=%d %s" % (act, "scale" if with_scale else "no scale"), run,
+                [Tol("out", "out", y, S, 2 if with_scale else 1)])
+
+
+def gated_bn_cases():
+    return [_gated_bn(act, s, 900 + 2 * act + s) for act in (0, 1, 2) for s in (False, True)]
+
+
+# ---------------------------------------------------------------------------------------------------- max pool (HMR)
+def _maxpool(edge, seed, n, c, h, w, k, s):
+    x = _randn(_gen(seed), n, c, h, w)
+    ref = _nhwc(F.max_pool2d(x, kernel_size=k, stride=s, ceil_mode=True)).contiguous()
+
+    def run(api, put, alloc):
+        out = alloc(_full(tuple(ref.shape)))
+        api.maxpool_nchw_to_nhwc(put(x), k, s, out=out)
+        return {"out": out, "allocated": api.maxpool_nchw_to_nhwc(put(x), k, s)}
+    return Case("maxpool_nchw_to_nhwc", edge, run, [Bits("out", "out", ref), Bits("allocated", "allocated", ref)])
+
+
+def maxpool_cases():
+    return [_maxpool("112 -> 56 clipped last window", 1001, 1, 3, 112, 112, 3, 2),
+            _maxpool("h = k", 1002, 2, 4, 3, 5, 3, 2),
+            _maxpool("k < stride", 1003, 2, 3, 4, 5, 1, 2)]                      # torch: 2 x 3 windows, not 3 x 3
+
+
+# ---------------------------------------------------------------------------------------------- global average pool
+def _avgpool(edge, seed, n, h, w, c, ld, scale, relu):
+    g = _gen(seed)
+    x = _randn(g, n, h, w, c, scale=2.0)
+    sc, sh = (_randn(g, c, scale=0.3, shift=1.0), _randn(g, c, scale=0.5)) if scale else (None, None)
+    v = x.double() * sc.double() + sh.double() if scale else x.double()
+    Sv = (x.double() * sc.double()).abs() + sh.double().abs() if scale else x.double().abs()
+    if relu:
+        v = v.clamp(min=0)
+    init = _full((n, ld))
+
+    def run(api, put, alloc):
+        buf = alloc(init)
+        api.global_avgpool_nhwc(put(x), put(sc) if scale else None, put(sh) if scale else None, relu=relu, out=buf, ld_out=ld)
+        return {"out": buf[:, :c], "pad": buf[:, c:]}
+    return Case("global_avgpool_nhwc", edge, run, [Tol("out", "out", v.mean(dim=(1, 2)), Sv.mean(dim=(1, 2)), 2 * h * w + 1),
+                                                   Bits("columns >= c untouched", "pad", init[:, c:])])
+
+
+def avgpool_cases():
+    return [_avgpool("scale relu ld_out > c", 1101, 2, 7, 7, 40, 48, True, True),
+            _avgpool("no scale hw=1", 1102, 3, 1, 1, 20, 20, False, False),
+            _avgpool("scale no relu", 1103, 1, 5, 9, 70, 70, True, False)]
+
+
+# ----------------------------------------------------------------------------------------------------------- linear
+def _linear(edge, seed, n, k, m, ld_x=None, ld_out=None, bias=True, relu=False, acc=False):
+    g = _gen(seed)
+    ld_x, ld_out = ld_x or k, ld_out or m
+    xfull = _randn(g, n, ld_x)
+    wt = _randn(g, m, k, scale=k ** -0.5)
+    b = _randn(g, m) if bias else None
+    init = _randn(g, n, ld_out) if acc else _full((n, ld_out))
+    x = xfull[:, :k].double()
+    y = x @ wt.double().t() + (b.double() if bias else 0.0)
+    S = x.abs() @ wt.double().abs().t() + (b.double().abs() if bias else 0.0)
+    if relu:
+        y = y.clamp(min=0)
+    if acc:
+        y, S = y + init[:, :m].double(), S + init[:, :m].double().abs()
+
+    def run(api, put, alloc):
+        buf = alloc(init)
+        api.linear(put(xfull)[:, :k], put(wt), put(b) if bias else None, relu=relu, out=buf[:, :m], accumulate=acc)
+        return {"out": buf[:, :m], "pad": buf[:, m:]}
+    return Case("linear", edge, run, [Tol("out", "out", y, S, k + 2), Bits("columns >= m untouched", "pad", init[:, m:])])
+
+
+def linear_cases():
+    return [_linear("k=1", 1201, 3, 1, 5, relu=True),
+            _linear("k=31 ld_x > k bias None", 1202, 2, 31, 7, ld_x=40, bias=False),
+            _linear("k=85 m=1 ld_out > m", 1203, 4, 85, 1, ld_out=3, relu=True),
+            _linear("k=2133", 1204, 2, 2133, 9, relu=True),
+            # HMR's third regressor layer: theta += fc3(h2), theta a column slice of [features | theta]
+            _linear("accumulate into a slice", 1205, 2, 1024, 85, ld_out=2133, acc=True)]
+
+
+# ----------------------------------------------------------------------------------------------------------- LPIPS
+_LPIPS_SHIFT, _LPIPS_SCALE = (-.030, -.088, -.188), (.458, .448, .450)
+
+
+def _lpips_input(from01, seed):
+    g = _gen(seed)
+    n, h, w = 2, 5, 7
+    lo = 0.0 if from01 else -1.0
+    pred = torch.rand(n, 3, h, w, generator=g) * (1 - lo) + lo
+    ref = torch.rand(n, 3, h, w, generator=g) * (1 - lo) + lo
+    pred[0, :, 0, :2], ref[1, :, 4, 6] = lo, 1.0                   # the ends of the range
+    x = torch.cat([pred, ref])
+    if from01:
+        x = x * 2 - 1
+    want = (x - torch.tensor(_LPIPS_SHIFT).view(1, 3, 1, 1)) / torch.tensor(_LPIPS_SCALE).view(1, 3, 1, 1)
+
+    def run(api, put, alloc):
+        out = alloc(_full((2 * n, 3, h, w)))
+        api.lpips_input(put(pred), put(ref), from01=from01, out=out)
+        return {"out": out}
+    return Case("lpips_input", "from01=%d" % from01, run, [Bits("out", "out", want)])
+
+
+def _lpips_layer(edge, seed, n, h, w, c, layer, L=3):
+    g = _gen(seed)
+    feat = _randn(g, 2 * n, h, w, c).clamp(min=0) * 3                 # post-ReLU features
+    if h * w > 1:
+        feat[n + 1, 0, 1] = 0.0                                        # one ref pixel all zero, its pred pixel not
+    lin = torch.rand(c, generator=g) * 0.2
+    layers0 = _randn(g, n, L)
+    score0 = _randn(g, n).abs()
+    f = feat.double()
+    fn = f / (f.pow(2).sum(-1, keepdim=True).sqrt() + 1e-10)
+    d = fn[n:] - fn[:n]
+    v = (d * d * lin.double()).sum(-1).mean(dim=(1, 2))
+    Sv = ((fn[n:].abs() + fn[:n].abs()) ** 2 * lin.double()).sum(-1).mean(dim=(1, 2))
+    score = v + score0.double() if layer > 0 else v
+    Ss = Sv + score0.double().abs() if layer > 0 else Sv
+    others = [k for k in range(L) if k != layer]
+
+    def run(api, put, alloc):
+        layers, sc = alloc(layers0), alloc(score0)
+        api.lpips_layer(put(feat), put(lin), layer, layers, sc)
+        return {"layer": layers[:, layer], "others": layers[:, others], "score": sc}
+    return Case("lpips_layer", edge, run, [Tol("layers[:, %d]" % layer, "layer", v, Sv, c * h * w),
+                                           Bits("other layers untouched", "others", layers0[:, others]),
+                                           Tol("score", "score", score, Ss, c * h * w + 1)])
+
+
+def lpips_cases():
+    return [_lpips_input(False, 1301), _lpips_input(True, 1302),
+            _lpips_layer("c=40 zero pixel layer 0", 1303, 2, 5, 7, 40, 0),
+            _lpips_layer("hw=1 layer 2 accumulates", 1304, 3, 1, 1, 40, 2)]
+
+
+# ------------------------------------------------------------------------------------------------- layout / warp
+def _nhwc_to_nchw(edge, seed, n, h, w, c, cs):
+    x = _randn(_gen(seed), n, h, w, cs)
+
+    def run(api, put, alloc):
+        out = alloc(_full((n, c, h, w)))
+        api.nhwc_to_nchw(put(x), c=c, out=out)
+        return {"out": out}
+    return Case("nhwc_to_nchw", edge, run, [Bits("out", "out", _nchw(x[..., :c]).contiguous())])
+
+
+def _warp_nchw(edge, seed, sb, B, C, h, w, th, tw, ac, acc):
+    g = _gen(seed)
+    x = _randn(g, sb, C, h, w)
+    T = _flow(g, B, th, tw)
+    init = _randn(g, B, C, h, w) if acc else _full((B, C, h, w))
+    ref, S = _warp64(x, T, h, w, ac, B)
+    if acc:
+        ref, S = ref + init.double(), S + init.double().abs()
+
+    def run(api, put, alloc):
+        out = alloc(init)
+        api.warp_nchw(put(x), put(T), align_corners=bool(ac), out=out, accumulate=acc)
+        return {"out": out}
+    return Case("warp_nchw", edge, run, [Tol("out", "out", ref, S, 5 if acc else 4)])
+
+
+def layout_warp_cases():
+    return [_nhwc_to_nchw("c=4 c_stride=32", 1401, 2, 3, 5, 4, 32),
+            _nhwc_to_nchw("c=100 hw=37x3", 1402, 2, 37, 3, 100, 104),
+            _warp_nchw("accumulate src_batch=B C=70", 1403, 2, 2, 70, 9, 13, 16, 16, 1, True),
+            _warp_nchw("src_batch=1 T same size", 1404, 1, 3, 5, 12, 7, 12, 7, 0, False)]
+
+
+CASES = (norm_act_cases() + instance_stats_cases() + heads_cases() + frames_out_cases() + conv_direct_cases()
+         + heads7x7_cases() + gated_bn_cases() + maxpool_cases() + avgpool_cases() + linear_cases() + lpips_cases()
+         + layout_warp_cases())
+
+# The edges each front-end must be exercised at; one case each.
+REQUIRED_EDGES = {
+    "norm_act_nhwc": ["stats c=%d" % c for c in (8, 16, 64, 128, 256, 512, 1024, 2048)] + [
+        "affine gamma+beta", "affine gamma only", "affine beta only", "bare", "stats relu residual", "bare warp",
+        "EXT post affine res_step 2", "EXT res_step 2", "lo_format 1 c=512"] + [
+        "warp sb=%s T %s ac=%d" % (sb, t, ac) for sb in ("1", "n") for t in ("same", "larger") for ac in (0, 1)] + [
+        "range %s" % v for v in ("1023.7", "1023.75", "1024", "-1024", "59984", "59990", "60000", "65520", "+inf", "-inf",
+                                 "nan")],
+    "instance_stats_nhwc": ["hw=35 c=40", "hw=1000 c=96", "hw=16640 c=33"],
+    "heads_composite": ["kw=%d w=%d c_stride=%d bg_batch=%s" % (kw, w, cs, b) for w in (1, 2, 3, 70)
+                        for kw, cs, b in ((0, 4, "1"), (0, 32, "n"), (7, 32, "1"), (7, 32, "n"))] + [
+        "u8 sweep", "range 8.0", "range below 8.0", "range -8.0", "range nan"],
+    "frames_out": ["u8 sweep"],
+    "conv2d_direct_nchw": ["cout=7", "dilation 2", "stride 2 odd sizes", "pad > k/2", "bias None", "1x1", "inpaintor 5x5",
+                           "inpaintor 4x4 s2", "inpaintor 3x3 dil 16"],
+    "conv7x7_heads_nhwc": ["1x1", "5x3", "17x65"],
+    "gated_bn_nchw": ["act=%d %s" % (a, s) for a in (0, 1, 2) for s in ("no scale", "scale")],
+    "maxpool_nchw_to_nhwc": ["112 -> 56 clipped last window", "h = k", "k < stride"],
+    "global_avgpool_nhwc": ["scale relu ld_out > c", "no scale hw=1", "scale no relu"],
+    "linear": ["k=1", "k=31 ld_x > k bias None", "k=85 m=1 ld_out > m", "k=2133", "accumulate into a slice"],
+    "lpips_input": ["from01=0", "from01=1"],
+    "lpips_layer": ["c=40 zero pixel layer 0", "hw=1 layer 2 accumulates"],
+    "nhwc_to_nchw": ["c=4 c_stride=32", "c=100 hw=37x3"],
+    "warp_nchw": ["accumulate src_batch=B C=70", "src_batch=1 T same size"],
+}
+
+# Front-ends the emulator replaces whose kernels are tested elsewhere: name -> "file::test function".
+COVERED_ELSEWHERE = {
+    "ConvPlan": "test_conv_gpu.py::test_conv2d",
+    "pack_conv_weight": "test_conv_emulation_gpu.py::test_pack_conv_weight_bits",
+    "pack_conv_weight_rowk": "test_conv_emulation_gpu.py::test_pack_conv_weight_rowk_bits",
+    "nchw_to_nhwc_split": "test_conv_emulation_gpu.py::test_nchw_to_nhwc_split_bits",
+    "pack_head_weights": "test_conv_gpu.py::test_heads_7x7",
+    "gated_act_nhwc": "test_inpaintor_ops_gpu.py::test_gated_epilogue_matches_torch",
+    "self_attention_nhwc": "test_inpaintor_ops_gpu.py::test_self_attention_matches_torch",
+    "det_bias_act": "test_detector_kernels_gpu.py::test_bias_act",
+    "conv2d_direct_relu_nhwc": "test_metrics_gpu.py::test_stem_11x11_s4_matches_conv2d",
+    "maxpool_nhwc": "test_metrics_gpu.py::test_floor_pool_nhwc_exact",
+    "maxpool_nhwc_slice": "test_inception_gpu.py::test_maxpool_slice_exact",
+    "bn_act_segment": "test_inception_gpu.py::test_bn_act_segment_matches_float64",
+    "inception_input": "test_inception_gpu.py::test_input_matches_interpolate",
+    "correspond": "test_raster_gpu.py::test_correspond_matches_oracle",
+    "_correspond": "test_raster_gpu.py::test_correspond_matches_oracle",
+}
+
+
+def verify(case, outs, kernel):
+    """Run the case's checks on CPU outputs; kernel=False skips the checks of kernel-only formats."""
+    for chk in case.checks:
+        if kernel or not chk.kernel_only:
+            chk(case.name, outs)

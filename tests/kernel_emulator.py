@@ -134,9 +134,11 @@ def norm_act_nhwc(raw, stats, gamma, beta, relu, ws, eps=1e-5, residual=None, wa
         y_f32.copy_(v)
     _emit(ops, None, y_hi, y_lo)
     if range_flag is not None and y_hi is not None:
-        m = float(ops.abs().max())
-        if m >= 1024:
-            range_flag |= 3 if m >= 60000 else 1
+        a = ops.half().float().abs()                # the bits describe the emitted fp16 hi operand
+        if bool(((a >= 60000) | torch.isnan(a)).any()):
+            range_flag |= 3
+        elif bool((a >= 1024).any()):
+            range_flag |= 1
 
 
 def nchw_to_nhwc_split(x, c_pad=None, pad_hw=(0, 0, 0, 0), hi=None, lo=None, split=True):
@@ -259,11 +261,9 @@ def heads_composite(raw, bg=None, want_color=True, want_mask=True, color=None, m
         r = torch.zeros(n, h, w, 4)
         for kx in range(folded_kw):
             sh = kx - folded_kw // 2                       # out[y, x] += raw[y, x + sh, kx*4 : kx*4+4]
-            src = raw[..., kx * 4:kx * 4 + 4]
-            if sh >= 0:
-                r[:, :, :w - sh] += src[:, :, sh:]
-            else:
-                r[:, :, -sh:] += src[:, :, :w + sh]
+            x0, x1 = max(0, -sh), min(w, w - sh)           # (no column inside the image when w <= |sh|)
+            if x1 > x0:
+                r[:, :, x0:x1] += raw[:, :, x0 + sh:x1 + sh, kx * 4:kx * 4 + 4]
     else:
         r = raw[..., :4]
     col = torch.tanh(r[..., :3]).permute(0, 3, 1, 2)
@@ -280,6 +280,10 @@ def heads_composite(raw, bg=None, want_color=True, want_mask=True, color=None, m
             outs.append(val.contiguous() if val is not None else None)
     if pred_hwc is not None:
         pred_hwc.copy_(p.permute(0, 2, 3, 1))
+    if pred_u8 is not None:                                  # float32 ((img + 1) / 2.0 * 255) truncated, BGR
+        pred_u8.copy_(((p.permute(0, 2, 3, 1) + 1) / 2.0 * 255).to(torch.uint8).flip(-1))
+    if range_flag is not None and bool((~(r.abs() < 8)).any()):
+        range_flag |= 4                                      # a pre-activation of magnitude >= 8, or NaN
     return tuple(outs)
 
 
@@ -299,6 +303,9 @@ def correspond(cam, verts, face_idx, image_size, map_fn, src_p2verts, src_img=No
 
 def warp_nchw(x, T, align_corners=None, out=None, accumulate=False):
     ac = K.default_align_corners() if align_corners is None else align_corners
+    h, w = x.shape[2:]
+    if tuple(T.shape[1:3]) != (h, w):                       # the flow is resized to the image (align_corners=True)
+        T = F.interpolate(T.permute(0, 3, 1, 2), size=(h, w), mode='bilinear', align_corners=True).permute(0, 2, 3, 1)
     y = torch.nn.functional.grid_sample(x.expand(T.shape[0], -1, -1, -1), T, mode='bilinear', padding_mode='zeros',
                                         align_corners=ac)
     if out is not None:

@@ -37,6 +37,20 @@ def test_bad_sizes_rejected(L):
     assert L.lwb_raster_workspace_bytes(2, 256, 100) == 2 * 256 * 256 * 8 + 16 + 2 * 100 * 4
 
 
+def test_direct_conv_rejects_an_empty_output(L):
+    """h + 2p - d(k-1) - 1 in [-(s-1), -1]: floor division gives no output row, C's truncating division one."""
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("dummy pointers: an accepted call would launch on the visible GPU")
+    dummy = ctypes.c_void_p(1024)
+    # n, cin, h, w, cout, kh, kw, stride, pad, dil: 2 + 0 - 2 - 1 = -1 rows at stride 2, then the same for columns
+    for h, w in ((2, 8), (8, 2)):
+        rc = L.lwb_conv2d_direct_nchw(dummy, dummy, None, 1, 3, h, w, 4, 3, 3, 2, 0, 1, dummy, None)
+        assert rc == -1 and b"empty output" in L.lwb_last_error(), (h, w, rc, L.lwb_last_error())
+    rc = L.lwb_conv2d_direct_nchw(dummy, dummy, None, 1, 3, 8, 8, 4, 3, 3, 3, 0, 4, dummy, None)     # 8 - 8 - 1 = -1, dil 4
+    assert rc == -1 and b"empty output" in L.lwb_last_error()
+
+
 def test_conv_plan_argument_checks(L):
     d = _lib.ConvDesc(n=1, h_in=32, w_in=32, h_out=32, w_out=32, cin0=60, cin1=0, cout=64, kh=3, kw=3, stride=1, pad=1,
                       dil=1, transposed=0, split=1, rowk=0, row_pitch=0, n_tile=0, halo=0)
