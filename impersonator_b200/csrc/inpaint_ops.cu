@@ -51,7 +51,8 @@ __global__ void __launch_bounds__(256) k_gated_act(GatedParams P)
             if (P.act == 2) a = a > 0.f ? a : 0.2f * a;
             out = a * (1.f / (1.f + expf(-gt)));
             if (P.scale) out = fmaf(out, __ldg(P.scale + ch), __ldg(P.shift + ch));
-            if (P.clamp) out = fminf(fmaxf(out, -1.f), 1.f);
+            // torch.clamp (networks/inpaintor.py:187,196) keeps a NaN; fminf / fmaxf would return -1 for it
+            if (P.clamp) out = out > 1.f ? 1.f : (out < -1.f ? -1.f : out);
         }
         v[k] = out;
     }

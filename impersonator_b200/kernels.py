@@ -479,6 +479,8 @@ def gated_act_nhwc(raw, c, bias, act, scale, shift, upsample=1, clamp=False, y_f
     for t in (y_f32, y_hi):
         if t is not None and tuple(t.shape[:3]) != (n, h * u, w * u):
             raise LwbError("gated_act: output grid must be [n, %d, %d, *]" % (h * u, w * u))
+    if y_lo is not None and y_hi is not None and y_lo.shape != y_hi.shape:
+        raise LwbError("gated_act: y_lo is %s, y_hi is %s" % (tuple(y_lo.shape), tuple(y_hi.shape)))
     _count(1)
     check(lib().lwb_gated_act_nhwc(ptr(raw), n, h, w, int(c), cs, ptr(bias), int(act), ptr(scale), ptr(shift), u, 1 if clamp else 0,
                                    ptr(y_f32), y_f32.shape[3] if y_f32 is not None else 0, ptr(y_hi), ptr(y_lo),
@@ -492,8 +494,14 @@ def self_attention_nhwc(qkv, bias, x, gamma, dq=16, out=None):
     _chk_cuda(qkv, bias, x, gamma, out)
     n, h, w, ld = qkv.shape
     dv = x.shape[3]
+    if tuple(x.shape[:3]) != (n, h, w):
+        raise LwbError("self_attention: x is %s, qkv has [n, h, w] = %s" % (tuple(x.shape), (n, h, w)))
+    if tuple(bias.shape) != (2 * int(dq) + dv,):
+        raise LwbError("self_attention: bias must be [%d], got %s" % (2 * int(dq) + dv, tuple(bias.shape)))
     if out is None:
         out = torch.empty_like(x)
+    elif out.shape != x.shape:
+        raise LwbError("self_attention: out must be %s, got %s" % (tuple(x.shape), tuple(out.shape)))
     _count(1)
     check(lib().lwb_self_attention_nhwc(ptr(qkv), ld, ptr(bias), n, h * w, int(dq), dv, ptr(x), ptr(gamma), ptr(out), stream()),
           "lwb_self_attention_nhwc")

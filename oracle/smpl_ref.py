@@ -26,40 +26,43 @@ def rodrigues(theta):                                    # :64-101
     outer = r[:, :, None] * r[:, None, :]
     z = torch.zeros_like(r[:, 0])
     skew = torch.stack([z, -r[:, 2], r[:, 1], r[:, 2], z, -r[:, 0], -r[:, 1], r[:, 0], z], dim=1).view(-1, 3, 3)
-    return c * torch.eye(3)[None] + (1 - c) * outer + s * skew
+    return c * torch.eye(3, dtype=theta.dtype)[None] + (1 - c) * outer + s * skew
 
 
 def rigid_chain(Rs, Js, parents, rotate_base=False):    # :129-218
     N = Rs.shape[0]
     root = Rs[:, 0]
     if rotate_base:
-        root = root @ torch.diag(torch.tensor([1., -1., -1.]))
+        root = root @ torch.diag(torch.tensor([1., -1., -1.], dtype=Rs.dtype))
 
     def make_A(R, t):
         top = torch.cat([R, t[:, :, None]], dim=2)
-        return torch.cat([top, torch.tensor([0., 0., 0., 1.]).expand(N, 1, 4)], dim=1)
+        return torch.cat([top, torch.tensor([0., 0., 0., 1.], dtype=R.dtype).expand(N, 1, 4)], dim=1)
 
     res = [make_A(root, Js[:, 0])]
     for i in range(1, parents.shape[0]):
         res.append(res[parents[i]] @ make_A(Rs[:, i], Js[:, i] - Js[:, parents[i]]))
     res = torch.stack(res, dim=1)
     new_J = res[:, :, :3, 3]
-    init_bone = res @ torch.cat([Js, torch.zeros(N, 24, 1)], dim=2)[..., None]
+    init_bone = res @ torch.cat([Js, Js.new_zeros(N, 24, 1)], dim=2)[..., None]
     A = res - torch.nn.functional.pad(init_bone, (3, 0))
     return new_J, A
 
 
 def forward(m, beta, theta, rotate_base=False):          # :285-375 -> verts, joints, Rs, J_transformed
+    """In the dtype of beta / theta: model tensors of another float dtype are cast (float64 runs the oracle as a
+    float64 reference of the kernel)."""
+    m = {k: (v.to(beta.dtype) if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in m.items()}
     N = beta.shape[0]
     V = m['v_template'].shape[0]
     v_shaped = (beta @ m['shapedirs']).view(N, V, 3) + m['v_template']
     J = torch.stack([v_shaped[:, :, d] @ m['J_regressor'] for d in range(3)], dim=2)
     Rs = rodrigues(theta.reshape(-1, 3)).view(N, 24, 3, 3)
-    pose_feature = (Rs[:, 1:] - torch.eye(3)).reshape(N, 207)
+    pose_feature = (Rs[:, 1:] - torch.eye(3, dtype=Rs.dtype)).reshape(N, 207)
     v_posed = (pose_feature @ m['posedirs']).view(N, V, 3) + v_shaped
     J_transformed, A = rigid_chain(Rs, J, m['parents'], rotate_base)
     T = (m['weights'][None].expand(N, -1, -1) @ A.view(N, 24, 16)).view(N, V, 4, 4)
-    v_h = torch.cat([v_posed, torch.ones(N, V, 1)], dim=2)[..., None]
+    v_h = torch.cat([v_posed, v_posed.new_ones(N, V, 1)], dim=2)[..., None]
     verts = (T @ v_h)[:, :, :3, 0]
     joints = torch.stack([verts[:, :, d] @ m['joint_regressor'] for d in range(3)], dim=2)
     return verts, joints, Rs, J_transformed

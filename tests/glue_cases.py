@@ -29,20 +29,43 @@ def _get(outs, out):
 
 
 class Tol(object):
-    def __init__(self, label, out, ref, S, K, tau=TAU, unit=U32, kernel_only=False):
-        self.label, self.out, self.ref, self.S, self.K = label, out, ref.double(), S.double(), K
-        self.tau, self.unit, self.kernel_only = tau, unit, kernel_only
+    """``guard=False`` drops the tenth-of-one-term assertion for bars that grow with K (the attention sums), whose
+    strength is shown by mutants instead.  A NaN reference wants NaN, an infinite one the same infinity.  ``ref`` and
+    ``S`` may be functions, evaluated at the first check (the large references are not built at import)."""
 
-    def __call__(self, case, outs):
+    def __init__(self, label, out, ref, S, K, tau=TAU, unit=U32, kernel_only=False, guard=True):
+        self.label, self.out, self._ref, self._S, self.K = label, out, ref, S, K
+        self.tau, self.unit, self.kernel_only, self.guard = tau, unit, kernel_only, guard
+
+    @property
+    def ref(self):
+        if callable(self._ref):
+            self._ref = self._ref()
+        return self._ref.double()
+
+    @property
+    def S(self):
+        if callable(self._S):
+            self._S = self._S()
+        return self._S.double()
+
+    def ratio(self, case, outs):
+        """-> the elementwise err / bar of the outputs (inf where a NaN or infinity is not matched)."""
         got = _get(outs, self.out).double()
         assert got.shape == self.ref.shape, "%s/%s: shape %s, want %s" % (case, self.label, tuple(got.shape), tuple(self.ref.shape))
         tol = self.tau * self.unit * self.S
-        pos = self.S > 0
-        assert bool((tol[pos] < 0.1 * self.S[pos] / self.K).all()), \
+        pos = (self.S > 0) & torch.isfinite(self.S)
+        assert not self.guard or bool((tol[pos] < 0.1 * self.S[pos] / self.K).all()), \
             "%s/%s: tol %g * S is not below a tenth of one of the %d terms" % (case, self.label, self.tau * self.unit, self.K)
         err = (got - self.ref).abs()
         ratio = torch.where(tol > 0, err / tol.clamp(min=1e-300), torch.where(err > 0, float("inf"), 0.0))
-        ratio = torch.where(torch.isnan(err), float("inf"), ratio)
+        ratio = torch.where(torch.isnan(err) | torch.isnan(ratio), float("inf"), ratio)
+        same = (got == self.ref) | (torch.isnan(got) & torch.isnan(self.ref))
+        return torch.where(same, 0.0, ratio), err
+
+    def __call__(self, case, outs):
+        ratio, err = self.ratio(case, outs)
+        err = torch.where(torch.isnan(err), 0.0, err)
         r = float(ratio.max()) if ratio.numel() else 0.0
         print("%s/%s: max err %.3g, max err/tol %.3f (K=%d)" % (case, self.label, float(err.max()) if err.numel() else 0.0, r, self.K))
         assert r <= 1.0, "%s/%s: error %.3g times the bar at %s" % (case, self.label, r, tuple(int(i) for i in np.unravel_index(
@@ -612,9 +635,452 @@ def layout_warp_cases():
             _warp_nchw("src_batch=1 T same size", 1404, 1, 3, 5, 12, 7, 12, 7, 0, False)]
 
 
+# ------------------------------------------------------------------------------------------------ self attention
+ATT_DQ, ATT_DV = 16, 128
+ATT_SIZES = {1: (1, 1), 63: (7, 9), 64: (8, 8), 65: (5, 13), 129: (3, 43), 4096: (64, 64)}
+
+
+def attention64(qkv, bias, x, gamma, dq=ATT_DQ):
+    """gamma * softmax(q k^T) v + x in float64, and its S: the same sums on |v| and |x| with the softmax weights
+    unchanged.  -> (ref, S) as [n, h, w, dv]."""
+    n, h, w, _ = qkv.shape
+    dv = x.shape[3]
+    t = (qkv[..., :2 * dq + dv].double() + bias.double()).view(n, h * w, -1)
+    q, k, v = t[..., :dq], t[..., dq:2 * dq], t[..., 2 * dq:]
+    p = torch.softmax(torch.bmm(q, k.transpose(1, 2)), dim=-1)
+    g, xd = gamma.double(), x.double().view(n, h * w, dv)
+    ref = g * torch.bmm(p, v) + xd
+    S = g.abs() * torch.bmm(p, v.abs()) + xd.abs()
+    return ref.view(n, h, w, dv), S.view(n, h, w, dv)
+
+
+def _attention(edge, seed, n, N, qk="rand", ld=ATT_DQ * 2 + ATT_DV, gamma=0.7, zero_x=False, nan_pad=False):
+    """qk: rand (logits about +-5) | uniform (q = 0) | big_first / big_last (one key 30 above the rest, in the first tile
+    or in the last, partial one) | ascending (every key's logit above the last, for every query) | span80 (logits
+    spread over +-80: most exp terms underflow) | ties (four distinct keys, each repeated)."""
+    g = _gen(seed)
+    h, w = ATT_SIZES[N]
+    qkv = _randn(g, n, h, w, ld)
+    bias = _randn(g, ATT_DQ * 2 + ATT_DV, scale=0.1)
+    x = torch.zeros(n, h, w, ATT_DV) if zero_x else _randn(g, n, h, w, ATT_DV)
+    q, k = qkv[..., :ATT_DQ], qkv[..., ATT_DQ:2 * ATT_DQ]              # views: edits land in qkv
+    if qk == "rand":
+        q.mul_(0.6)
+    elif qk == "uniform":
+        q.copy_(-bias[:ATT_DQ].expand_as(q))                             # q + bias_q = 0 exactly: every logit is 0
+    else:
+        # every query a positive multiple of one direction u: a key's logit order is the same for all queries
+        u = _randn(g, ATT_DQ)
+        u = u / u.norm()
+        q.copy_(u * (0.5 + torch.rand(n, h, w, 1, generator=g)) - bias[:ATT_DQ])
+        t = torch.randn(n, N, generator=g)
+        if qk in ("big_first", "big_last"):
+            t[:, 0 if qk == "big_first" else N - 1] = 30.0
+        elif qk == "ascending":
+            t = torch.linspace(-4, 4, N).expand(n, N).clone()
+        elif qk == "span80":
+            t = torch.linspace(-80, 80, N)[torch.randperm(N, generator=g)].expand(n, N).clone()
+        elif qk == "ties":
+            t = torch.tensor([1.5, -0.5, 1.5, 0.25])[torch.arange(N) % 4].expand(n, N).clone()
+        kk = t[..., None] * u + 0.05 * _randn(g, n, N, ATT_DQ) * (qk not in ("ties", "ascending"))
+        k.copy_(kk.view(n, h, w, ATT_DQ) - bias[ATT_DQ:2 * ATT_DQ])
+    if nan_pad:
+        qkv[..., 2 * ATT_DQ + ATT_DV:] = NAN
+    gm = torch.tensor([gamma])
+    ref_S = []
+
+    def ref(i):                                          # built at the first check, not at import
+        if not ref_S:
+            ref_S.extend(attention64(qkv, bias, x, gm))
+        return ref_S[i]
+
+    def run(api, put, alloc):
+        out = alloc(_full((n, h, w, ATT_DV)))
+        api.self_attention_nhwc(put(qkv), put(bias), put(x), put(gm), out=out)
+        return {"out": out}
+    if gamma == 0:
+        return Case("self_attention_nhwc", edge, run, [Bits("out == x", "out", x)])
+    # The kernel sums the N keys one after the other in fp32: the weights l and each accumulator channel are sequential
+    # sums of N terms, every term rescaled by a running product of up to N factors exp(m_old - m_new).  The deterministic
+    # bound of such a sum is about N u S (Higham's gamma_N); tau = 16 covers the logit's own 16-term dot, the exp
+    # evaluations and the final fmaf.  At N = 4096 the bar is no longer below one term (the tenth-of-a-term guard cannot
+    # hold), so test_attention_mutants_cpu.py shows on these cases that a dropped tile, a missed rescale or a mixed-up
+    # value slot each exceed it.
+    return Case("self_attention_nhwc", edge, run, [Tol("out", "out", lambda: ref(0), lambda: ref(1), N, tau=TAU * N,
+                                                                    guard=False)])
+
+
+def attention_cases():
+    cases = [_attention("N=%d" % N, 1500 + N % 100, 2, N) for N in (1, 63, 64, 65, 129, 4096)]
+    cases += [
+        _attention("N=65 n=3", 1510, 3, 65),
+        _attention("uniform logits", 1511, 2, 129, qk="uniform"),
+        _attention("big key in the first tile", 1512, 2, 129, qk="big_first"),
+        _attention("big key in the last partial tile", 1513, 2, 129, qk="big_last"),
+        _attention("ascending logits", 1514, 2, 129, qk="ascending"),
+        _attention("logits span +-80", 1515, 2, 129, qk="span80"),
+        _attention("exact ties", 1516, 2, 129, qk="ties"),
+        _attention("gamma=0", 1517, 2, 65, gamma=0.0),
+        _attention("gamma<0", 1518, 2, 65, gamma=-1.3),
+        _attention("x=0", 1519, 2, 65, zero_x=True),
+        _attention("ld=176 NaN pad", 1520, 2, 65, ld=176, nan_pad=True),
+    ]
+    return cases
+
+
+ATTENTION_EDGES = ["N=%d" % N for N in (1, 63, 64, 65, 129, 4096)] + [
+    "N=65 n=3", "uniform logits", "big key in the first tile", "big key in the last partial tile", "ascending logits",
+    "logits span +-80", "exact ties", "gamma=0", "gamma<0", "x=0", "ld=176 NaN pad"]
+
+
+# -------------------------------------------------------------------------------------------------- gated epilogue
+def _pin_nan(got, want):
+    """``want`` with its NaN entries replaced by ``got``'s where that is NaN too: any NaN payload is the same NaN."""
+    both = torch.isnan(want.float()) & torch.isnan(got.float())
+    return torch.where(both, got, want)
+
+
+def _up2(t, up):
+    return t.repeat_interleave(up, dim=1).repeat_interleave(up, dim=2) if up == 2 else t
+
+
+def _gated(edge, seed, n, h, w, c, cs, up=1, outputs="f32 hi lo", lo_format=0, bias=True, act=2, scale=True, clamp=False,
+           f32_extra=0, c_pad=None, raw=None, gates=None, flag=None, wide=1.0):
+    """outputs: the buffers passed (f32 and / or operands hi [+ lo]); f32_extra: columns of the f32 buffer past c, which
+    must keep their sentinel; gates: values written over the first gate channels; flag: the range_flag bits wanted."""
+    g = _gen(seed)
+    outs_on = outputs.split()
+    c_pad = c_pad or ((c + 63) // 64 * 64)
+    if raw is None:
+        raw = _randn(g, n, h, w, cs, scale=2.0 * wide)
+    if gates is not None:
+        flat = raw[..., c:2 * c].reshape(-1)
+        flat[:len(gates)] = torch.tensor(gates)
+        raw[..., c:2 * c] = flat.view(n, h, w, c)
+    b = _randn(g, 2 * c, scale=0.3) if bias else None
+    sc, sh = (_randn(g, c, scale=0.3, shift=1.0), _randn(g, c, scale=0.2)) if scale else (None, None)
+
+    rd = raw.double()
+    a, gt = rd[..., :c], rd[..., c:2 * c]
+    Sa, Sg = a.abs(), gt.abs()
+    if bias:
+        a, gt = a + b.double()[:c], gt + b.double()[c:]
+        Sa, Sg = Sa + b.double()[:c].abs(), Sg + b.double()[c:].abs()
+    if act == 2:
+        Sa = torch.where(a < 0, 0.2 * Sa, Sa)
+        a = F.leaky_relu(a, 0.2)
+    sig = torch.sigmoid(gt)
+    # d sigmoid = sigmoid (1 - sigmoid) d gate; expf(-gate) overflows below a gate of -88.7, where the kernel's 0 is
+    # within 2^-127 of the sigmoid: 2^-100 * tau * u covers that
+    dsig = torch.where(sig * (1 - sig) > 0, sig * (1 - sig) * Sg, torch.zeros_like(sig))
+    y, S = a * sig, Sa * (sig + dsig + 2.0 ** -100)
+    if scale:
+        y, S = y * sc.double() + sh.double(), S * sc.double().abs() + sh.double().abs()
+    if clamp:
+        y = y.clamp(-1, 1)
+    y, S = _up2(y, up), _up2(S, up)
+    ho, wo = h * up, w * up
+    init_f32 = _full((n, ho, wo, c + f32_extra))
+
+    def call(api, put, alloc, o, f32, hi, lo):
+        api.gated_act_nhwc(put(raw), c, put(b), act, put(sc), put(sh), upsample=up, clamp=clamp, y_f32=f32, y_hi=hi, y_lo=lo,
+                           lo_format=lo_format, range_flag=o.get("flag"))
+
+    def run(api, put, alloc):
+        o = {}
+        if flag is not None:
+            o["flag"] = alloc(torch.zeros(1, dtype=torch.int32))
+        if "f32" in outs_on:
+            o["f32"] = alloc(init_f32)
+        if "hi" in outs_on:
+            o["hi"] = alloc(_full((n, ho, wo, c_pad), dtype=torch.float16))
+            if "lo" in outs_on:
+                o["lo"] = alloc(_full((n, ho, wo, c_pad), dtype=torch.float16))
+        call(api, put, alloc, o, o.get("f32"), o.get("hi"), o.get("lo"))
+        if "f32" not in outs_on:              # the same call with an f32 output: the value the operands must split
+            o["f32"] = alloc(init_f32)
+            call(api, put, alloc, {}, o["f32"], None, None)
+        return o
+
+    checks = [Tol("y_f32", lambda o: o["f32"][..., :c], y, S, 3)]
+    if f32_extra:
+        checks.append(Bits("f32 columns >= c untouched", lambda o: o["f32"][..., c:], init_f32[..., c:]))
+    if flag is not None:
+        checks.append(Flag(flag))
+    if "hi" in outs_on:
+        def v_pad(o):
+            v = torch.zeros(n, ho, wo, c_pad)
+            v[..., :c] = o["f32"][..., :c]
+            return v
+        checks.append(Bits("hi", "hi", lambda o: _pin_nan(o["hi"], fp16_pair(v_pad(o))[0])))
+        if "lo" in outs_on and lo_format == 0:
+            checks.append(Bits("lo", "lo", lambda o: _pin_nan(o["lo"], fp16_pair(v_pad(o))[1])))
+        elif "lo" in outs_on:
+            def lo8(o):
+                from test_conv_emulation_gpu import pair_blocks
+                v = v_pad(o)
+                return pair_blocks(v / 16, (v - v.half().float()) * 1024)
+            checks.append(Bits("lo8", lambda o: o["lo"].view(torch.uint8), lo8))
+    return Case("gated_act_nhwc", edge, run, checks)
+
+
+def inpaintor_gated_bindings():
+    """Every (c, c_stride, up, outputs, lo_format) the inpaintor binds at 256x256 in the three precision modes, from
+    _InpaintStream over InpaintSANet's module tree.  CPU only: needs kernel_emulator's stand-ins installed."""
+    from impersonator_b200.inpaintor import InpaintSANet, _InpaintStream
+    net = InpaintSANet(c_dim=4).eval()
+    combos = set()
+    for split in (0, 1, 2):
+        st = _InpaintStream(net, 1, 256, 256, torch.device("cpu"), split)
+        for r in st.coarse + st.refine + st.upsample:
+            outs = ["f32"] if r["y_f32"] is not None else []
+            if r["out"] is not None:
+                outs += ["hi"] + (["lo"] if r["out"].lo is not None else [])
+            combos.add((r["c"], r["conv"].out.shape[3], r["up"], " ".join(outs), st.lo_format))
+    return sorted(combos)
+
+
+# (c, c_stride, up, outputs, lo_format) of inpaintor_gated_bindings(); test_glue_cases_cpu.py checks the list is complete
+INPAINTOR_GATED = [
+    (3, 16, 1, "f32", 0), (3, 16, 1, "f32", 1),
+    (16, 32, 1, "hi", 0), (16, 32, 1, "hi lo", 0), (16, 32, 1, "hi lo", 1),
+    (32, 64, 1, "hi", 0), (32, 64, 1, "hi lo", 0), (32, 64, 1, "hi lo", 1),
+    (64, 128, 1, "hi", 0), (64, 128, 1, "hi lo", 0), (64, 128, 1, "hi lo", 1),
+    (64, 128, 2, "hi", 0), (64, 128, 2, "hi lo", 0), (64, 128, 2, "hi lo", 1),
+    (128, 256, 1, "hi", 0), (128, 256, 1, "hi lo", 0), (128, 256, 1, "hi lo", 1),
+    (128, 256, 1, "f32 hi", 0), (128, 256, 1, "f32 hi lo", 0), (128, 256, 1, "f32 hi lo", 1),
+    (128, 256, 2, "hi", 0), (128, 256, 2, "hi lo", 0), (128, 256, 2, "hi lo", 1),
+]
+
+
+def _binding_edge(cb):
+    return "inpaintor c=%d c_stride=%d up=%d %s lo_format=%d" % cb
+
+
+# fp16 of the emitted value and the bits wanted, as norm_act's range cases
+RANGE_VALUES = (("1023.7", 1023.7, 0), ("1023.75", 1023.75, 1), ("1024", 1024.0, 1), ("-1024", -1024.0, 1),
+                ("59984", 59984.0, 1), ("59990", 59990.0, 3), ("60000", 60000.0, 3), ("65520", 65520.0, 3),
+                ("+inf", float("inf"), 3), ("-inf", float("-inf"), 3), ("nan", NAN, 3))
+
+
+def _gated_range(edge, v, want, outputs="f32 hi lo"):
+    """act none, no bias / scale, gate +inf (sigmoid exactly 1): y = a exactly, one channel of one pixel at v."""
+    raw = torch.rand(1, 3, 5, 16, generator=_gen(1600)) * 8 - 4
+    raw[..., 8:] = float("inf")
+    raw[0, 1, 2, 5] = v
+    return _gated(edge, 1600, 1, 3, 5, 8, 16, outputs=outputs, bias=False, act=0, scale=False, raw=raw, flag=want)
+
+
+def gated_cases():
+    cases = [_gated(_binding_edge(cb), 1700 + i, 2, 5, 7, cb[0], cb[1], up=cb[2], outputs=cb[3], lo_format=cb[4],
+                    scale=cb[0] != 3, act=0 if cb[0] == 3 else 2, clamp=cb[0] == 3, wide=2.0 if cb[0] == 3 else 1.0)
+             for i, cb in enumerate(INPAINTOR_GATED)]
+    cases += [
+        _gated("c=3 f32 only", 1801, 2, 4, 6, 3, 8, outputs="f32"),
+        _gated("c=16 f32 only f32_stride=21", 1802, 2, 4, 6, 16, 40, outputs="f32", f32_extra=5),
+        _gated("c=3 f32_stride=8", 1803, 1, 3, 5, 3, 6, outputs="f32", f32_extra=5),
+        _gated("up=2 odd h w lo_format=0", 1804, 2, 5, 7, 24, 48, up=2, lo_format=0),
+        _gated("up=2 odd h w lo_format=1", 1805, 2, 5, 7, 24, 48, up=2, lo_format=1),
+        _gated("no bias", 1806, 2, 3, 5, 16, 32, bias=False),
+        _gated("no scale", 1807, 2, 3, 5, 16, 32, scale=False),
+        _gated("act none", 1808, 2, 3, 5, 16, 32, act=0),
+        _gated("clamp beyond +-1", 1809, 2, 3, 5, 16, 32, clamp=True, wide=3.0),
+        _gated("bare", 1810, 2, 3, 5, 16, 32, bias=False, scale=False, act=0),
+        _gated("gates +-100 +-inf nan", 1811, 1, 3, 5, 16, 32, clamp=True, flag=3,
+               gates=[100.0, -100.0, float("inf"), float("-inf"), NAN, 89.0, -89.0, -88.0]),
+    ]
+    cases += [_gated_range("range %s" % label, v, want) for label, v, want in RANGE_VALUES]
+    cases.append(_gated_range("range 65520 no operand output", 65520.0, 0, outputs="f32"))
+    return cases
+
+
+GATED_EDGES = [_binding_edge(cb) for cb in INPAINTOR_GATED] + [
+    "c=3 f32 only", "c=16 f32 only f32_stride=21", "c=3 f32_stride=8", "up=2 odd h w lo_format=0", "up=2 odd h w lo_format=1",
+    "no bias", "no scale", "act none", "clamp beyond +-1", "bare", "gates +-100 +-inf nan"] + [
+    "range %s" % label for label, _, _ in RANGE_VALUES] + ["range 65520 no operand output"]
+
+
+# ------------------------------------------------------------------------------------------------------------- SMPL
+SMPL_PARENTS = [-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21]    # depth 9 (0..22)
+SMPL_NJ, SMPL_NPF, SMPL_NREG = 24, 207, 19
+SMPL_TAU = 2
+
+
+def smpl_model(seed, V, nb=10, sparse=False, blend=4.0):
+    """A seeded random SMPL model in the oracle's layout (float32 values): 24 joints, 207 pose bases; dense skin
+    weights, or two joints per vertex when sparse.  blend scales the blend shapes above the synthetic model's
+    (|shapedirs| ~ 0.03, |posedirs| ~ 0.017), so that dropping one beta or a quarter of the pose terms moves the vertices
+    by more than 10 bars (test_smpl_cases_cpu.py)."""
+    g = _gen(seed)
+    w = torch.rand(V, SMPL_NJ, generator=g) ** 4
+    if sparse:
+        keep = torch.zeros(V, SMPL_NJ, dtype=torch.bool)
+        for _ in range(2):
+            keep[torch.arange(V), torch.randint(SMPL_NJ, (V,), generator=g)] = True
+        w = torch.where(keep, w + 0.1, torch.zeros_like(w))
+    jr = torch.rand(V, SMPL_NJ, generator=g)
+    reg = torch.zeros(V, SMPL_NREG)
+    for j in range(SMPL_NREG):                                   # each output joint from at most 4 vertices
+        reg[torch.randint(V, (4,), generator=g), j] = torch.rand(4, generator=g) * 0.5
+    return dict(v_template=_randn(g, V, 3, scale=0.3), shapedirs=_randn(g, nb, V * 3, scale=0.03 * blend),
+                J_regressor=jr / jr.sum(0, keepdim=True), posedirs=_randn(g, SMPL_NPF, V * 3, scale=0.017 * blend),
+                parents=np.array(SMPL_PARENTS, dtype=np.int32), weights=w / w.sum(1, keepdim=True), joint_regressor=reg)
+
+
+def smpl_device_model(m):
+    """The kernel's model dict: impersonator_b200.smpl.SMPL._device_model's folding of the joint regression."""
+    V, nb = m["v_template"].shape[0], m["shapedirs"].shape[0]
+    Jr = m["J_regressor"].double().t()
+    js = torch.einsum('jv,kvd->jdk', Jr, m["shapedirs"].double().view(nb, V, 3)).reshape(72, nb)
+    return dict(v_template=m["v_template"].contiguous(), shapedirs=m["shapedirs"].contiguous(),
+                posedirs=m["posedirs"].contiguous(), weights=m["weights"].contiguous(),
+                j_template=(Jr @ m["v_template"].double()).float().contiguous(), j_shapedirs=js.float().contiguous(),
+                parents=torch.tensor(SMPL_PARENTS, dtype=torch.int32), joint_regressor_t=m["joint_regressor"].t().contiguous())
+
+
+def smpl_bars(m, beta, theta, rotate_base, cam):
+    """S of every smpl_forward output, in units of u: a first-order forward error analysis of the kernel's fp32
+    operations, evaluated on the float64 values.
+
+    Entrywise |.| products of the 9 rotations along a chain grow like 3^9, far above any real error, because a rotation
+    does not grow an error vector.  So the chain is bounded in 2-norms: E_i bounds the spectral norm of the error of the
+    global rotation of joint i, T_i the norm of the error of its translation.  Rotating an error keeps its norm, so
+    along the chain E_i = E_parent + e_R(i) + 9 adds up.  Here e_R is 3x the largest entry bound of Rodrigues' error,
+    and 9 is the 3x3 product's rounding (3-term dots of unit rows and columns).  So the bar grows linearly with the
+    chain depth (at most 9 levels), not geometrically.  Each operation counts one u on the magnitudes it combines:
+      Rodrigues  8 (|c| I + |1 - c| |r r^T| + |s| |[r]x| + angle + 1): the fp32 angle is a few ulps of itself off, and
+                 cosf / sinf an ulp of 1
+      joints J   nb + 2 on |J_reg|^T (|v_template| + |shapedirs|^T |beta|) (the folded fp32 regression, nb fma)
+      v_posed    56 on |pf| |posedirs| (52 fma per K slice + the adds), nb + 3 on the shape blend and template
+      skinning   24 + 4 on (|w| |A|) [|v_posed|; 1] (the 24-joint sum, then the 4-term product)
+      joints     ceil(V / 128) + 7 on |reg|^T |verts| (128 thread-strided sums and a 7-level tree)
+    SMPL_TAU = 2 leaves room for the second-order terms."""
+    from oracle import smpl_ref
+    d = lambda t: torch.as_tensor(t).double()                    # noqa: E731
+    N, V, nb = beta.shape[0], m["v_template"].shape[0], beta.shape[1]
+    vt, sd, pd, Jreg, W, reg = (d(m[k]) for k in ("v_template", "shapedirs", "posedirs", "J_regressor", "weights",
+                                                   "joint_regressor"))
+    b = beta.double()
+    t = theta.double().view(N, SMPL_NJ, 3)
+    angle = torch.norm(t + 1e-8, dim=2, keepdim=True)
+    r = t / angle
+    c, s = torch.cos(angle)[..., None], torch.sin(angle)[..., None]
+    ra = r.abs()
+    skew = torch.stack([torch.zeros_like(ra[..., 0]), ra[..., 2], ra[..., 1], ra[..., 2], torch.zeros_like(ra[..., 0]),
+                        ra[..., 0], ra[..., 1], ra[..., 0], torch.zeros_like(ra[..., 0])], dim=-1).view(N, SMPL_NJ, 3, 3)
+    SR = 8 * (c.abs() * torch.eye(3, dtype=torch.float64) + (1 - c).abs() * ra[..., :, None] * ra[..., None, :]
+              + s.abs() * skew + (angle + 1)[..., None])
+    Rs = smpl_ref.rodrigues(t.reshape(-1, 3)).view(N, SMPL_NJ, 3, 3)
+    v_shaped = (b @ sd).view(N, V, 3) + vt
+    J = torch.stack([v_shaped[:, :, k] @ Jreg for k in range(3)], dim=2)                     # [N, 24, 3]
+    SJ = torch.stack([((b.abs() @ sd.abs()).view(N, V, 3)[:, :, k] + vt.abs()[:, k]) @ Jreg.abs() for k in range(3)], dim=2)
+    jerr = (nb + 2) * SJ.norm(dim=2)                                                        # [N, 24]
+    pf = (Rs[:, 1:] - torch.eye(3, dtype=torch.float64)).reshape(N, SMPL_NPF)
+    v_posed = (pf @ pd).view(N, V, 3) + v_shaped
+    SV = (56 * (pf.abs() @ pd.abs()) + SR[:, 1:].reshape(N, SMPL_NPF) @ pd.abs()).view(N, V, 3) \
+        + (nb + 3) * ((b.abs() @ sd.abs()).view(N, V, 3) + vt.abs())
+    # the chain on true values, with E (rotation) and T (translation) error norms
+    root = Rs[:, 0] @ torch.diag(torch.tensor([1., -1., -1.], dtype=torch.float64)) if rotate_base else Rs[:, 0]
+    eR = 3 * SR.amax(dim=(2, 3))
+    Gr, Gt, E, T = [root], [J[:, 0]], [eR[:, 0]], [jerr[:, 0]]
+    for i in range(1, SMPL_NJ):
+        p = SMPL_PARENTS[i]
+        dJ = J[:, i] - J[:, p]
+        tl = dJ.norm(dim=1)
+        Gr.append(Gr[p] @ Rs[:, i])
+        Gt.append((Gr[p] @ dJ[..., None])[..., 0] + Gt[p])
+        E.append(E[p] + eR[:, i] + 9)
+        T.append(T[p] + E[p] * tl + jerr[:, i] + jerr[:, p] + J[:, i].norm(dim=1) + J[:, p].norm(dim=1)
+                 + 7 * (tl + Gt[p].norm(dim=1)))
+    Gr, Gt, E, T = torch.stack(Gr, 1), torch.stack(Gt, 1), torch.stack(E, 1), torch.stack(T, 1)
+    At = Gt - (Gr @ J[..., None])[..., 0]                                                   # A's translation column
+    TA = T + E * J.norm(dim=2) + jerr + 7 * (J.norm(dim=2) + Gt.norm(dim=2))
+    A_abs = torch.cat([Gr.abs(), At.abs()[..., None]], dim=3).reshape(N, SMPL_NJ, 12)
+    skin = (W.abs()[None] @ A_abs).view(N, V, 3, 4)
+    Sskin = (skin[..., :3] @ v_posed.abs()[..., None])[..., 0] + skin[..., 3]
+    prop = (W[None] * E[:, None, :]).sum(-1) * v_posed.norm(dim=2) + (W[None] * TA[:, None, :]).sum(-1)
+    S_verts = prop[..., None] + SV.norm(dim=2, keepdim=True) + 28 * Sskin
+    verts = smpl_ref.forward(m, beta.double(), theta.double(), rotate_base=rotate_base)[0]
+    rabs = reg.abs()
+    S_joints = torch.stack([S_verts[:, :, k] @ rabs + ((V + 127) // 128 + 7) * (verts[:, :, k].abs() @ rabs)
+                            for k in range(3)], dim=2)
+    joints = torch.stack([verts[:, :, k] @ reg for k in range(3)], dim=2)
+    cd = cam.double()
+    S_j2d = cd[:, None, 0:1].abs() * (S_joints[..., :2] + 2 * (joints[..., :2].abs() + cd[:, None, 1:].abs()))
+    return dict(verts=S_verts, joints=S_joints, Rs=SR, Jt=T[..., None].expand(N, SMPL_NJ, 3), j2d=S_j2d)
+
+
+def _smpl(edge, seed, batch, V=33, nb=10, rotate_base=False, sparse=False, angles=None, wild=False, nan_joint=None):
+    g = _gen(seed)
+    m = smpl_model(seed, V, nb, sparse)
+    beta = _randn(g, batch, nb)
+    theta = _randn(g, batch, 72, scale=0.4)
+    if wild:
+        theta = (torch.rand(batch, 72, generator=g) * 2 - 1) * np.pi
+    if angles is not None:                               # joint j of every frame at angles[j % len] about a random axis
+        ax = _randn(g, batch, SMPL_NJ, 3).double()
+        ax = ax / ax.norm(dim=2, keepdim=True)
+        a = torch.tensor(angles, dtype=torch.float64)[torch.arange(SMPL_NJ) % len(angles)]
+        theta = (ax * a[None, :, None]).float().reshape(batch, 72)
+    if nan_joint is not None:                            # theta + 1e-8 = 0 in fp32: angle 0, r = -inf, the frame is NaN
+        theta[batch // 2, nan_joint * 3:nan_joint * 3 + 3] = -1e-8
+    cam = torch.cat([torch.rand(batch, 1, generator=g) + 0.5, _randn(g, batch, 2, scale=0.2)], dim=1)
+    dm = smpl_device_model(m)
+    built = {}
+
+    def refs():                                          # built at the first check, not at import
+        if not built:
+            from oracle import smpl_ref
+            verts, joints, Rs, Jt = smpl_ref.forward(m, beta.double(), theta.double(), rotate_base=rotate_base)
+            ref = dict(verts=verts, joints=joints, Rs=Rs, Jt=Jt, j2d=smpl_ref.orth_proj_idrot(joints, cam.double()))
+            if nan_joint is not None:                    # NaN exactly where the float32 oracle (the reference model) is NaN
+                v32, j32, R32, J32 = smpl_ref.forward(m, beta, theta, rotate_base=rotate_base)
+                r32 = dict(verts=v32, joints=j32, Rs=R32, Jt=J32, j2d=smpl_ref.orth_proj_idrot(j32, cam))
+                ref = {k: torch.where(torch.isnan(r32[k].double()), float("nan"), v) for k, v in ref.items()}
+            built["ref"] = ref
+            built["S"] = smpl_bars(m, beta, theta, rotate_base, cam)
+        return built
+
+    def run(api, put, alloc):
+        v, j, R, J, p = api.smpl_forward(put(beta), put(theta), {k: put(t) for k, t in dm.items()}, rotate_base=rotate_base,
+                                         cam=put(cam))
+        return dict(verts=v, joints=j, Rs=R, Jt=J, j2d=p)
+
+    def tol(label, key, K):
+        return Tol(label, key, lambda: refs()["ref"][key], lambda: refs()["S"][key], K, tau=SMPL_TAU)
+    reg_terms = int((m["joint_regressor"] != 0).sum(0).max())
+    case = Case("smpl_forward", edge, run, [tol("Rs", "Rs", 3), tol("J_transformed", "Jt", 4 * 9),
+                                            tol("verts", "verts", SMPL_NPF + nb + SMPL_NJ), tol("joints", "joints", reg_terms),
+                                            tol("j2d", "j2d", reg_terms + 1)], emulated=False)
+    case.smpl = (m, beta, theta, rotate_base, cam, refs)
+    return case
+
+
+def smpl_cases():
+    cases = [_smpl("batch=%d" % b, 1900 + b, b) for b in (1, 7, 8, 9, 16, 17)]
+    cases += [
+        _smpl("V=1", 1921, 3, V=1),
+        _smpl("V=31 sparse weights", 1922, 3, V=31, sparse=True),
+        _smpl("V=33 sparse weights", 1923, 9, V=33, sparse=True),
+        _smpl("V=6890", 1924, 9, V=6890),
+        _smpl("num_betas=1", 1925, 3, nb=1),
+        _smpl("num_betas=16", 1926, 3, nb=16),
+        _smpl("rotate_base", 1927, 9, rotate_base=True),
+        _smpl("angles 0 1e-6 pi 2pi 3.5pi", 1928, 3, angles=[0.0, 1e-6, np.pi, 2 * np.pi, 3.5 * np.pi]),
+        _smpl("wild poses", 1929, 9, wild=True, rotate_base=True),
+        _smpl("NaN frame", 1930, 3, nan_joint=13),
+    ]
+    return cases
+
+
+SMPL_EDGES = ["batch=%d" % b for b in (1, 7, 8, 9, 16, 17)] + [
+    "V=1", "V=31 sparse weights", "V=33 sparse weights", "V=6890", "num_betas=1", "num_betas=16", "rotate_base",
+    "angles 0 1e-6 pi 2pi 3.5pi", "wild poses", "NaN frame"]
+
+
 CASES = (norm_act_cases() + instance_stats_cases() + heads_cases() + frames_out_cases() + conv_direct_cases()
          + heads7x7_cases() + gated_bn_cases() + maxpool_cases() + avgpool_cases() + linear_cases() + lpips_cases()
-         + layout_warp_cases())
+         + layout_warp_cases() + attention_cases() + gated_cases() + smpl_cases())
 
 # The edges each front-end must be exercised at; one case each.
 REQUIRED_EDGES = {
@@ -640,6 +1106,9 @@ REQUIRED_EDGES = {
     "lpips_layer": ["c=40 zero pixel layer 0", "hw=1 layer 2 accumulates"],
     "nhwc_to_nchw": ["c=4 c_stride=32", "c=100 hw=37x3"],
     "warp_nchw": ["accumulate src_batch=B C=70", "src_batch=1 T same size"],
+    "self_attention_nhwc": ATTENTION_EDGES,
+    "gated_act_nhwc": GATED_EDGES,
+    "smpl_forward": SMPL_EDGES,
 }
 
 # Front-ends the emulator replaces whose kernels are tested elsewhere: name -> "file::test function".
@@ -649,8 +1118,6 @@ COVERED_ELSEWHERE = {
     "pack_conv_weight_rowk": "test_conv_emulation_gpu.py::test_pack_conv_weight_rowk_bits",
     "nchw_to_nhwc_split": "test_conv_emulation_gpu.py::test_nchw_to_nhwc_split_bits",
     "pack_head_weights": "test_conv_gpu.py::test_heads_7x7",
-    "gated_act_nhwc": "test_inpaintor_ops_gpu.py::test_gated_epilogue_matches_torch",
-    "self_attention_nhwc": "test_inpaintor_ops_gpu.py::test_self_attention_matches_torch",
     "det_bias_act": "test_detector_kernels_gpu.py::test_bias_act",
     "conv2d_direct_relu_nhwc": "test_metrics_gpu.py::test_stem_11x11_s4_matches_conv2d",
     "maxpool_nhwc": "test_metrics_gpu.py::test_floor_pool_nhwc_exact",

@@ -192,7 +192,26 @@ def gated_act_nhwc(raw, c, bias, act, scale, shift, upsample=1, clamp=False, y_f
         y = y.clamp(-1, 1)
     if upsample == 2:
         y = y.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
-    _emit(y, y_f32, y_hi, y_lo)
+    if y_f32 is not None:
+        y_f32[..., :c] = y                          # columns c.. of a wider f32 buffer are left alone
+    if y_hi is None:
+        return
+    _emit(y, None, y_hi, y_lo if lo_format == 0 else None)
+    if y_lo is not None and lo_format == 1:
+        # the e4m3 pair blocks: per 64 channels, 64 bytes of e4m3(y / 16) then 64 bytes of e4m3((y - hi) * 1024)
+        v = torch.zeros(y_hi.shape)
+        v[..., :c] = y
+        e4m3 = lambda t: t.clamp(-448, 448).to(torch.float8_e4m3fn).view(torch.uint8)      # noqa: E731
+        lead, cp = v.shape[:-1], v.shape[-1]
+        blk = torch.stack([e4m3(v / 16).view(*lead, cp // 64, 64),
+                           e4m3((v - y_hi.float()) * 1024).view(*lead, cp // 64, 64)], dim=-2)
+        y_lo.view(torch.uint8).copy_(blk.reshape(*lead, 2 * cp))
+    if range_flag is not None:
+        a = y_hi.float().abs()                      # the bits describe the emitted fp16 hi operand
+        if bool(((a >= 60000) | torch.isnan(a)).any()):
+            range_flag |= 3
+        elif bool((a >= 1024).any()):
+            range_flag |= 1
 
 
 def self_attention_nhwc(qkv, bias, x, gamma, dq=16, out=None):

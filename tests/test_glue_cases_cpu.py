@@ -62,6 +62,15 @@ def test_every_emulated_front_end_is_covered():
     assert not problems, "\n".join(problems)
 
 
+def test_every_inpaintor_gated_binding_has_a_case(monkeypatch):
+    """The (c, c_stride, up, outputs, lo_format) of every gated epilogue the inpaintor binds at 256x256, in all three
+    precision modes, is one of the gated_act_nhwc cases."""
+    E.install(monkeypatch)
+    bound = G.inpaintor_gated_bindings()
+    print("\n".join(str(b) for b in bound))
+    assert bound == sorted(G.INPAINTOR_GATED)
+
+
 def test_cases_are_the_required_edges():
     names = [c.name for c in G.CASES]
     assert len(names) == len(set(names)), "duplicate case names"

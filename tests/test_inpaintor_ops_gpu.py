@@ -49,3 +49,32 @@ def test_gated_epilogue_matches_torch(cuda, c, c_stride, up, lo_format):
         assert float(hi[..., c:].float().abs().max()) == 0.0                       # zero-padded K channels
     if lo_format == 0:
         assert ((hi.float() + lo.float())[..., :c].cpu() - ref).abs().max().item() < 1e-5
+
+
+def _attention_args(cuda, n=1, h=3, w=5, dv=128):
+    return (torch.zeros(n, h, w, 160, device=cuda), torch.zeros(160, device=cuda), torch.zeros(n, h, w, dv, device=cuda),
+            torch.ones(1, device=cuda))
+
+
+@pytest.mark.parametrize("bad", ["x batch", "x grid", "bias length", "out shape"])
+def test_self_attention_rejects_mismatched_shapes(cuda, bad):
+    qkv, bias, x, gamma = _attention_args(cuda)
+    out = None
+    if bad == "x batch":
+        x = torch.zeros(2, 3, 5, 128, device=cuda)
+    elif bad == "x grid":
+        x = torch.zeros(1, 5, 3, 128, device=cuda)
+    elif bad == "bias length":
+        bias = torch.zeros(144, device=cuda)
+    else:
+        out = torch.zeros(1, 3, 4, 128, device=cuda)
+    with pytest.raises(K.LwbError):
+        K.self_attention_nhwc(qkv, bias, x, gamma, out=out)
+
+
+def test_gated_act_rejects_lo_of_another_shape(cuda):
+    raw = torch.zeros(1, 3, 5, 32, device=cuda)
+    hi = torch.zeros(1, 3, 5, 64, dtype=torch.float16, device=cuda)
+    lo = torch.zeros(1, 3, 4, 64, dtype=torch.float16, device=cuda)
+    with pytest.raises(K.LwbError):
+        K.gated_act_nhwc(raw, 16, None, 2, None, None, y_hi=hi, y_lo=lo)
