@@ -145,6 +145,19 @@ def stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+_OPEN = []                                                       # pin lists of the graph.CapturedStep objects being built
+
+
+def pin(obj):
+    """Called by every cache that hands out device buffers (the per-shape stream caches, binding.stream_for, and the
+    workspace caches of kernels): while a graph.CapturedStep is warming up / capturing, the object is also referenced by
+    that step, so that a later eviction or replacement in the cache cannot free buffers, plans or TMA descriptors the
+    captured graph still replays into."""
+    for keep in _OPEN:
+        keep.append(obj)
+    return obj
+
+
 def _chk_cuda(*ts):
     cur = None
     for t in ts:

@@ -325,9 +325,10 @@ __global__ void __launch_bounds__(256) k_resolve(RasterParams P)
     if (!P.tsf_inputs) return;
     const size_t plane = (size_t)is * is;
     float* out = P.tsf_inputs + (size_t)b * (3 + P.map_c) * plane + pn;
-    // models/imitator.py:259: tsf_img = F.grid_sample(src_img, T)
+    // models/imitator.py:259: tsf_img = F.grid_sample(src_img, T) over the whole image, background included: T = -2 there,
+    // which still reaches pixel 0 at image sizes 1 and 2 with align_corners (and no pixel from size 3 on)
     float rgb[3] = {0.f, 0.f, 0.f};
-    if (P.src_img && hit) {
+    if (P.src_img) {
         const float ix = unnormalize(tx, is, P.align_corners), iy = unnormalize(ty, is, P.align_corners);
         const float x0f = floorf(ix), y0f = floorf(iy);
         const int x0 = (int)x0f, y0 = (int)y0f, x1 = x0 + 1, y1 = y0 + 1;

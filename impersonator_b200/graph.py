@@ -14,18 +14,7 @@ import warnings
 import torch
 
 from . import kernels as K
-
-
-_OPEN = []                                                       # pin lists of the CapturedStep objects being built
-
-
-def pin(obj):
-    """Called by the per-shape stream caches (binding.stream_for) for every buffer-owning object they hand out: while
-    a CapturedStep is warming up / capturing, the object is also referenced by that step, so that a later LRU eviction from
-    the cache cannot free buffers, plans or TMA descriptors the captured graph still replays into."""
-    for keep in _OPEN:
-        keep.append(obj)
-    return obj
+from ._lib import _OPEN, pin  # noqa: F401 -- pin lives beside the library binding, which kernels' caches import too
 
 
 def graphs_enabled():

@@ -73,10 +73,11 @@ def project_to_faces(cam, vertices, faces_idx):
     return vertices_to_faces(verts, faces)
 
 
-def render_fim_wim(cam, vertices, faces_idx, image_size):
-    """SMPLRenderer.render_fim_wim (utils/nmr.py:263-278) -> f2verts, fim, wim (torch CPU)."""
+def render_fim_wim(cam, vertices, faces_idx, image_size, near=0.1, far=100.0):
+    """SMPLRenderer.render_fim_wim (utils/nmr.py:263-278) -> f2verts, fim, wim (torch CPU).  near / far: the nr
+    defaults, which the reference's renderer passes."""
     f2verts = project_to_faces(cam, vertices, faces_idx)
-    fim, wim, _ = raster.rasterize_fim_wim(f2verts.numpy(), image_size)      # near/far = nr defaults
+    fim, wim, _ = raster.rasterize_fim_wim(f2verts.numpy(), image_size, near, far)
     return f2verts, torch.from_numpy(fim), torch.from_numpy(wim)
 
 
@@ -125,11 +126,11 @@ def grid_sample(x, T, align_corners=True):
     return F.grid_sample(x, T, mode='bilinear', padding_mode='zeros', align_corners=align_corners)
 
 
-def correspond(cam, vertices, faces_idx, map_fn, src_p2v, src_img, image_size, align_corners=True):
+def correspond(cam, vertices, faces_idx, map_fn, src_p2v, src_img, image_size, align_corners=True, near=0.1, far=100.0):
     """models/imitator.py:251-260 (transfer_params_by_smpl) for a batch of target frames whose
-    source-side tables have batch 1: returns dict(fim, wim, cond, T, tsf_img, tsf_inputs, f2verts)."""
+    source-side tables have batch 1 (or one per frame): returns dict(fim, wim, cond, T, tsf_img, tsf_inputs, f2verts)."""
     bs = cam.shape[0]
-    f2verts, fim, wim = render_fim_wim(cam, vertices, faces_idx, image_size)
+    f2verts, fim, wim = render_fim_wim(cam, vertices, faces_idx, image_size, near, far)
     cond = encode_fim(fim, map_fn)
     T = cal_bc_transform(src_p2v.expand(bs, -1, -1, -1), fim, wim, image_size)
     tsf_img = grid_sample(src_img.expand(bs, -1, -1, -1), T, align_corners)

@@ -31,11 +31,13 @@ def _get(outs, out):
 class Tol(object):
     """``guard=False`` drops the tenth-of-one-term assertion for bars that grow with K (the attention sums), whose
     strength is shown by mutants instead.  A NaN reference wants NaN, an infinite one the same infinity.  ``ref`` and
-    ``S`` may be functions, evaluated at the first check (the large references are not built at import)."""
+    ``S`` may be functions, evaluated at the first check (the large references are not built at import); with
+    ``of_outputs`` they are functions of the outputs, evaluated at every check (contracts stated on the kernel's own
+    results, as Bits.want)."""
 
-    def __init__(self, label, out, ref, S, K, tau=TAU, unit=U32, kernel_only=False, guard=True):
+    def __init__(self, label, out, ref, S, K, tau=TAU, unit=U32, kernel_only=False, guard=True, of_outputs=False):
         self.label, self.out, self._ref, self._S, self.K = label, out, ref, S, K
-        self.tau, self.unit, self.kernel_only, self.guard = tau, unit, kernel_only, guard
+        self.tau, self.unit, self.kernel_only, self.guard, self.of_outputs = tau, unit, kernel_only, guard, of_outputs
 
     @property
     def ref(self):
@@ -52,15 +54,16 @@ class Tol(object):
     def ratio(self, case, outs):
         """-> the elementwise err / bar of the outputs (inf where a NaN or infinity is not matched)."""
         got = _get(outs, self.out).double()
-        assert got.shape == self.ref.shape, "%s/%s: shape %s, want %s" % (case, self.label, tuple(got.shape), tuple(self.ref.shape))
-        tol = self.tau * self.unit * self.S
-        pos = (self.S > 0) & torch.isfinite(self.S)
-        assert not self.guard or bool((tol[pos] < 0.1 * self.S[pos] / self.K).all()), \
+        ref, S = (self._ref(outs).double(), self._S(outs).double()) if self.of_outputs else (self.ref, self.S)
+        assert got.shape == ref.shape, "%s/%s: shape %s, want %s" % (case, self.label, tuple(got.shape), tuple(ref.shape))
+        tol = self.tau * self.unit * S
+        pos = (S > 0) & torch.isfinite(S)
+        assert not self.guard or bool((tol[pos] < 0.1 * S[pos] / self.K).all()), \
             "%s/%s: tol %g * S is not below a tenth of one of the %d terms" % (case, self.label, self.tau * self.unit, self.K)
-        err = (got - self.ref).abs()
+        err = (got - ref).abs()
         ratio = torch.where(tol > 0, err / tol.clamp(min=1e-300), torch.where(err > 0, float("inf"), 0.0))
         ratio = torch.where(torch.isnan(err) | torch.isnan(ratio), float("inf"), ratio)
-        same = (got == self.ref) | (torch.isnan(got) & torch.isnan(self.ref))
+        same = (got == ref) | (torch.isnan(got) & torch.isnan(ref))
         return torch.where(same, 0.0, ratio), err
 
     def __call__(self, case, outs):
@@ -80,8 +83,9 @@ class Bits(object):
         self.label, self.out, self.want, self.kernel_only = label, out, want, kernel_only
 
     def __call__(self, case, outs):
-        got = _get(outs, self.out).contiguous()
-        want = (self.want(outs) if callable(self.want) else self.want).contiguous()
+        dense = lambda t: torch.empty(t.shape, dtype=t.dtype).copy_(t)           # noqa: E731 -- unit strides, size-1 dims too
+        got = dense(_get(outs, self.out))
+        want = dense(self.want(outs) if callable(self.want) else self.want)
         assert got.dtype == want.dtype and got.shape == want.shape, "%s/%s: %s %s, want %s %s" % (
             case, self.label, got.dtype, tuple(got.shape), want.dtype, tuple(want.shape))
         g, w = got.view(torch.uint8), want.view(torch.uint8)
@@ -1078,9 +1082,11 @@ SMPL_EDGES = ["batch=%d" % b for b in (1, 7, 8, 9, 16, 17)] + [
     "angles 0 1e-6 pi 2pi 3.5pi", "wild poses", "NaN frame"]
 
 
+from correspond_cases import CORRESPOND_EDGES, RASTER_EDGES, correspond_cases, raster_cases  # noqa: E402 (uses the above)
+
 CASES = (norm_act_cases() + instance_stats_cases() + heads_cases() + frames_out_cases() + conv_direct_cases()
          + heads7x7_cases() + gated_bn_cases() + maxpool_cases() + avgpool_cases() + linear_cases() + lpips_cases()
-         + layout_warp_cases() + attention_cases() + gated_cases() + smpl_cases())
+         + layout_warp_cases() + attention_cases() + gated_cases() + smpl_cases() + correspond_cases() + raster_cases())
 
 # The edges each front-end must be exercised at; one case each.
 REQUIRED_EDGES = {
@@ -1109,6 +1115,8 @@ REQUIRED_EDGES = {
     "self_attention_nhwc": ATTENTION_EDGES,
     "gated_act_nhwc": GATED_EDGES,
     "smpl_forward": SMPL_EDGES,
+    "correspond": CORRESPOND_EDGES,
+    "raster_forward_face_index_map": RASTER_EDGES,
 }
 
 # Front-ends the emulator replaces whose kernels are tested elsewhere: name -> "file::test function".
@@ -1124,7 +1132,6 @@ COVERED_ELSEWHERE = {
     "maxpool_nhwc_slice": "test_inception_gpu.py::test_maxpool_slice_exact",
     "bn_act_segment": "test_inception_gpu.py::test_bn_act_segment_matches_float64",
     "inception_input": "test_inception_gpu.py::test_input_matches_interpolate",
-    "correspond": "test_raster_gpu.py::test_correspond_matches_oracle",
     "_correspond": "test_raster_gpu.py::test_correspond_matches_oracle",
 }
 

@@ -307,14 +307,21 @@ def heads_composite(raw, bg=None, want_color=True, want_mask=True, color=None, m
 
 
 def correspond(cam, verts, face_idx, image_size, map_fn, src_p2verts, src_img=None, align_corners=None,
-               want_f2verts=False, near=None, far=None, out=None):
-    """lwb_correspond's contract through the CPU oracle (oracle/nmr_ref.py + the C rasterizer restatement)."""
+               want_f2verts=False, near=K.NEAR, far=K.FAR, out=None):
+    """lwb_correspond's contract through the CPU oracle (oracle/nmr_ref.py + the C rasterizer restatement): one source
+    for every frame or one per frame, written into the caller's ``out`` buffers when given."""
     from oracle import nmr_ref
     ac = K.default_align_corners() if align_corners is None else align_corners
     img = src_img if src_img is not None else torch.zeros(1, 3, image_size, image_size)
-    c = nmr_ref.correspond(cam, verts, face_idx, map_fn, src_p2verts, img, image_size, align_corners=ac)
+    c = nmr_ref.correspond(cam, verts, face_idx, map_fn, src_p2verts, img, image_size, align_corners=ac, near=near, far=far)
     res = dict(fim=c["fim"], wim=c["wim"], T=c["T"], tsf_inputs=c["tsf_inputs"].contiguous(),
                f2verts=c["f2verts"] if want_f2verts else None)
+    if out is not None:
+        for k in ("fim", "wim", "T", "tsf_inputs"):
+            out[k].copy_(res[k])
+        if out.get("f2verts") is not None:
+            out["f2verts"].copy_(c["f2verts"])
+        res = out
     res["tsf_img"] = res["tsf_inputs"][:, :3]
     res["cond"] = res["tsf_inputs"][:, 3:]
     return res

@@ -231,3 +231,56 @@ def test_captured_graph_survives_stream_cache_eviction(cuda, net):
     torch.cuda.synchronize()
     assert torch.equal(img, want_img) and torch.equal(mask, want_mask)
     del junk
+
+
+def test_captured_graph_keeps_the_workspaces_it_replays_into(cuda):
+    """correspond and smpl_forward run on per-device cached workspaces, which a larger call replaces.  A step captured
+    around both (as the Imitator's chunk graph is) must keep the buffers it replays into (graph.pin) when an eager B = 16
+    call grows both caches; its replay then reproduces the eager result bit for bit and writes into no tensor allocated
+    after the growth."""
+    import glue_cases
+    from impersonator_b200 import kernels as K
+    from impersonator_b200.graph import CapturedStep
+    from impersonator_b200.nmr import SMPLRenderer
+    from oracle import nmr_ref
+    size = 256
+    v, f = S.uv_sphere()
+    r = SMPLRenderer(image_size=size, faces=f.numpy(), map_fn=S.synthetic_tables()["map_fn"]).to(cuda)
+    model = {k: t.to(cuda) for k, t in glue_cases.smpl_device_model(glue_cases.smpl_model(5, 6890)).items()}
+    cam_s, verts_s = S.synthetic_frames(1, seed=60, base_verts=v)
+    p2v = nmr_ref.src_p2verts(nmr_ref.project_to_faces(cam_s, verts_s, f)).contiguous().to(cuda)
+    src = S.synthetic_source(size).to(cuda)
+
+    def inputs(B, seed):
+        cam, verts = S.synthetic_frames(B, seed=seed, base_verts=v)
+        g = torch.Generator().manual_seed(seed)
+        return dict(cam=cam.to(cuda), verts=verts.to(cuda), beta=torch.randn(B, 10, generator=g).to(cuda),
+                    theta=(0.4 * torch.randn(B, 72, generator=g)).to(cuda))
+
+    def step_fn(cam, verts, beta, theta):
+        c = r.correspond(cam, verts, p2v, src)
+        sv, sj, _, _, _ = K.smpl_forward(beta, theta, model)
+        return c["fim"], c["wim"], c["T"], c["tsf_inputs"], sv, sj
+
+    small = inputs(2, 61)
+    idx = small["cam"].device.index
+    kinds = ("raster", "smpl")
+    for kind in kinds:                                   # start from empty caches: B = 2 sizes them, B = 16 grows them
+        K._ws_cache.pop((idx, kind), None)
+    want = [t.clone() for t in step_fn(**small)]
+    step = CapturedStep(step_fn, small)
+    assert step.captured
+    ptrs = {kind: K._ws_cache[(idx, kind)].data_ptr() for kind in kinds}
+    nbytes = {kind: K._ws_cache[(idx, kind)].numel() for kind in kinds}
+    step_fn(**inputs(16, 62))
+    torch.cuda.synchronize()
+    pinned = {t.data_ptr() for t in step.pinned if torch.is_tensor(t)}
+    for kind in kinds:
+        assert K._ws_cache[(idx, kind)].data_ptr() != ptrs[kind], "the B = 16 call did not replace the %s workspace" % kind
+        assert ptrs[kind] in pinned, "the captured step does not keep the %s workspace it replays into" % kind
+    junk = [torch.full((nbytes[kind],), 7, dtype=torch.uint8, device=cuda) for kind in kinds for _ in range(4)]
+    got = step(**small)
+    torch.cuda.synchronize()
+    for name, a, b in zip(("fim", "wim", "T", "tsf_inputs", "smpl verts", "smpl joints"), got, want):
+        assert torch.equal(a, b), name
+    assert all(bool((j == 7).all()) for j in junk), "the replay wrote into a tensor allocated after the capture"

@@ -221,3 +221,83 @@ def test_self_correspondence_is_the_identity_warp(cuda):
         assert (T[..., 0] - gx)[cov].abs().mean() < 2e-5
         assert torch.all(T[~cov] == -2) and torch.all(img[:, ~cov] == 0)
         assert (img - src[0])[:, cov].abs().max() < 5e-3
+
+
+def _correspond_args(cuda, B=2, s=16, F=4, V=5, C=3, sb=1):
+    return dict(cam=torch.ones(B, 3, device=cuda), verts=torch.zeros(B, V, 3, device=cuda),
+                face_idx=torch.zeros(F, 3, dtype=torch.int32, device=cuda), image_size=s,
+                map_fn=torch.zeros(F + 1, C, device=cuda), src_p2verts=torch.zeros(sb, F, 3, 2, device=cuda),
+                src_img=torch.zeros(sb, 3, s, s, device=cuda))
+
+
+def _correspond_out(cuda, B=2, s=16, F=4, C=3):
+    return dict(fim=torch.zeros(B, s, s, dtype=torch.int32, device=cuda), wim=torch.zeros(B, s, s, 3, device=cuda),
+                T=torch.zeros(B, s, s, 2, device=cuda), tsf_inputs=torch.zeros(B, 3 + C, s, s, device=cuda),
+                f2verts=torch.zeros(B, F, 3, 3, device=cuda))
+
+
+CORRESPOND_BAD = {
+    "cam [B,2]": lambda a, o, c: a.update(cam=torch.ones(2, 2, device=c)),
+    "cam of another batch": lambda a, o, c: a.update(cam=torch.ones(3, 3, device=c)),
+    "cam float64": lambda a, o, c: a.update(cam=torch.ones(2, 3, dtype=torch.float64, device=c)),
+    "verts [B,V,2]": lambda a, o, c: a.update(verts=torch.zeros(2, 5, 2, device=c)),
+    "face_idx [F,4]": lambda a, o, c: a.update(face_idx=torch.zeros(4, 4, dtype=torch.int32, device=c)),
+    "face_idx int64": lambda a, o, c: a.update(face_idx=torch.zeros(4, 3, dtype=torch.int64, device=c)),
+    "map_fn rows": lambda a, o, c: a.update(map_fn=torch.zeros(4, 3, device=c)),
+    "src_p2verts batch 3 of 2": lambda a, o, c: a.update(src_p2verts=torch.zeros(3, 4, 3, 2, device=c),
+                                                         src_img=torch.zeros(3, 3, 16, 16, device=c)),
+    "src_p2verts faces": lambda a, o, c: a.update(src_p2verts=torch.zeros(1, 5, 3, 2, device=c)),
+    "src_p2verts [sb,F,3,3]": lambda a, o, c: a.update(src_p2verts=torch.zeros(1, 4, 3, 3, device=c)),
+    "src_img of another size": lambda a, o, c: a.update(src_img=torch.zeros(1, 3, 32, 32, device=c)),
+    "src_img batch B, src_p2verts batch 1": lambda a, o, c: a.update(src_img=torch.zeros(2, 3, 16, 16, device=c)),
+    "src_img 4 channels": lambda a, o, c: a.update(src_img=torch.zeros(1, 4, 16, 16, device=c)),
+    "out fim shape": lambda a, o, c: o.update(fim=torch.zeros(2, 16, 15, dtype=torch.int32, device=c)),
+    "out fim float32": lambda a, o, c: o.update(fim=torch.zeros(2, 16, 16, device=c)),
+    "out wim shape": lambda a, o, c: o.update(wim=torch.zeros(2, 16, 16, 2, device=c)),
+    "out T shape": lambda a, o, c: o.update(T=torch.zeros(1, 16, 16, 2, device=c)),
+    "out tsf_inputs channels": lambda a, o, c: o.update(tsf_inputs=torch.zeros(2, 3, 16, 16, device=c)),
+    "out f2verts faces": lambda a, o, c: o.update(f2verts=torch.zeros(2, 3, 3, 3, device=c)),
+}
+
+
+@pytest.mark.parametrize("bad", sorted(CORRESPOND_BAD))
+def test_correspond_rejects_mismatched_shapes(cuda, bad):
+    """Every input and caller buffer is checked against the shapes the kernel indexes with (B, F, sb, image size): a
+    source image of another size or batch, or a short buffer, is an LwbError, not an out-of-bounds read or write."""
+    a, o = _correspond_args(cuda), _correspond_out(cuda)
+    CORRESPOND_BAD[bad](a, o, cuda)
+    with pytest.raises(K.LwbError):
+        K.correspond(a.pop("cam"), a.pop("verts"), a.pop("face_idx"), a.pop("image_size"), a.pop("map_fn"),
+                     a.pop("src_p2verts"), a.pop("src_img"), want_f2verts=True, out=o)
+
+
+RASTER_BAD = ["faces [B,F,3,2]", "faces [B,F,9]", "faces float64", "fim shape", "fim int64", "wim shape", "depth shape",
+              "faces_inv faces"]
+
+
+@pytest.mark.parametrize("bad", RASTER_BAD)
+def test_raster_forward_rejects_mismatched_shapes(cuda, bad):
+    B, F, s = 2, 4, 16
+    faces = torch.zeros(B, F, 3, 3, device=cuda)
+    fim = torch.full((B, s, s), -1, dtype=torch.int32, device=cuda)
+    wim = torch.zeros(B, s, s, 3, device=cuda)
+    depth = torch.zeros(B, s, s, device=cuda)
+    finv = torch.zeros(B, F, 3, 3, device=cuda)
+    if bad == "faces [B,F,3,2]":
+        faces = torch.zeros(B, F, 3, 2, device=cuda)
+    elif bad == "faces [B,F,9]":
+        faces = torch.zeros(B, F, 9, device=cuda)
+    elif bad == "faces float64":
+        faces = torch.zeros(B, F, 3, 3, dtype=torch.float64, device=cuda)
+    elif bad == "fim shape":
+        fim = torch.full((B, s, s + 1), -1, dtype=torch.int32, device=cuda)
+    elif bad == "fim int64":
+        fim = torch.full((B, s, s), -1, dtype=torch.int64, device=cuda)
+    elif bad == "wim shape":
+        wim = torch.zeros(B, s, s, device=cuda)
+    elif bad == "depth shape":
+        depth = torch.zeros(1, s, s, device=cuda)
+    else:
+        finv = torch.zeros(B, F + 1, 3, 3, device=cuda)
+    with pytest.raises(K.LwbError):
+        K.raster_forward_face_index_map(faces, fim, wim, depth, s, faces_inv=finv)
