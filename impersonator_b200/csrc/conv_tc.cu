@@ -11,22 +11,27 @@
 //           (out-of-bounds rows/cols are zero-filled by the TMA unit = the conv padding),
 //   W     = weights repacked once to [tap][Cout][Cin] fp16 (K-major rows of 128 bytes).
 // Both operands land in shared memory in the canonical K-major SWIZZLE_128B layout.  A CTA is one
-// producer warpgroup (one warp issues the TMA loads, see Regs) and two consumer warpgroups; each consumer
-// warpgroup owns 64 rows of the tile and issues, per tap and K = 64 chunk, 4 x wgmma (M64 x N_TILE x K16)
-// into register accumulators.
+// producer warpgroup (one warp issues the TMA loads, see Regs) and two consumer warpgroups that issue, per tap and K = 64
+// chunk, 4 x wgmma (K16) into register accumulators.
 //
 // Y-halo tap groups: one image row of the tile (8 px x 128 B) is exactly one 1024-byte swizzle atom, so
 // taps that read the same input view at the same dx with consecutive dy share ONE activation box of
-// TILE_H + cnt - 1 rows; tap i of the group starts its A descriptor i x 1024 B further in (the swizzle
+// TILE_H + cnt - 1 rows; tap i of the group starts its activation descriptor i x 1024 B further in (the swizzle
 // phase lives in address bits 7-9 and does not change).  The K loop runs (group, chunk, tap in group):
-// one A fetch per (group, chunk) into the A ring, one weight fetch per tap into the B ring.
+// one activation fetch per (group, chunk) into the A ring, one weight fetch per tap into the B ring.
 //
-// Swapped orientation (SWAP, every plan whose N tile is 64): the same 16K-output accumulator budget is spent as 64 output
-// channels x 256 pixels (32 x 8), with the channels on the wgmma M side: D^T[cout, pixel] = W[cout, K] . X[pixel, K]^T.
-// The [64][128 B] weight tile is the A operand and the activation box the B operand (both already K-major SWIZZLE_128B);
-// consumer warpgroup g issues M64 x N128 wgmmas on box rows 16 g .. 16 g + 15 (+ the tap's row offset).  Against an
-// N = 64 tile of 128 pixels this halves the weight fetches per FLOP and the per-tile overheads, and the wider wgmma reads
-// less shared memory per tensor-core cycle.
+// Channel-major orientation (every plan whose N tile is 64 or 128): the accumulator is D^T[cout, pixel] =
+// W[cout, K] . X[pixel, K]^T, with the channels on the wgmma M side.  The [N][128 B] weight tile is the A operand and the
+// activation box the B operand (both already K-major SWIZZLE_128B); each consumer warpgroup issues M64 x N128 wgmmas:
+//   N tile 128: 16 x 8-pixel tiles, warpgroup g takes weight rows 64 g .. 64 g + 63 and the whole 128-pixel window;
+//   N tile 64 : 32 x 8-pixel tiles (the same 16K-output accumulator budget), both warpgroups take all 64 weight rows,
+//               warpgroup g box rows 16 g .. 16 g + 15.
+// Each thread then holds two whole channels of its warpgroup's pixels.  With N tiles of 128 the two warpgroups hold
+// different channels, so a warpgroup's epilogue (stores and InstanceNorm statistics) needs nothing from the other one:
+// the warpgroup that finishes its K loop first goes on to the next tile's wgmmas, bounded only by the rings, and the
+// other's epilogue runs under them.  N = 64 tiles merge the two warpgroups' statistics (epilogue_channel_major).
+// N tiles of 16 / 32 (the folded heads) keep the pixel-major orientation: M = 128 pixels, warpgroup g tile rows
+// 8 g .. 8 g + 7, D[pixel, cout] = X . W^T with m64nNk16.
 //
 // Precision: x ~= x_hi + x_lo, w ~= w_hi + w_lo in fp16; with SPLIT the accumulator receives
 // x_hi*w_hi + x_hi*w_lo + x_lo*w_hi (fp32 accumulate), which reproduces the fp32 reference
@@ -44,7 +49,7 @@
 //                   NHWC8 row are 64 contiguous fp16, so one K = 64 stage covers a whole filter
 //                   row (overlapping-stride tensor map); 7 stages instead of 49.
 // Epilogue: accumulator registers -> fp32 NHWC global + per-(n, c) sum / sum of squares for the
-// InstanceNorm that follows every conv (lane shuffles -> smem -> one f64 atomic per column per tile).
+// InstanceNorm that follows every conv (f64 atomics).
 #include <cuda.h>
 
 #include <stdlib.h>
@@ -58,8 +63,8 @@
 namespace {
 
 constexpr int TILE_H = 16, TILE_W = 8;          // output pixels per tile (M = 128)
-constexpr int SWAP_N_TILE = 64;                  // plans with this N tile run the swapped orientation ...
-constexpr int SWAP_TILE_H = 32;                  // ... on 32 x 8 = 256-pixel tiles
+constexpr int SWAP_N_TILE = 64;                  // plans with this N tile run channel-major ...
+constexpr int SWAP_TILE_H = 32;                  // ... on 32 x 8 = 256-pixel tiles (N = 128: channel-major on 16 x 8)
 constexpr int KCHUNK = 64;                       // fp16 elements per K stage (128 B swizzle span)
 constexpr int ROW_BYTES = TILE_W * 128;          // one image row of an A box = one SWIZZLE_128B atom
 constexpr int MAX_TAPS = 49;
@@ -106,7 +111,10 @@ struct Cfg {
     static constexpr int B_BYTES = N_TILE * 128;
     static constexpr int B_STAGE_BYTES = B_BYTES * (SPLIT ? 2 : 1);
     static constexpr int BAR_BYTES = 4 * MAX_STAGES * 8;         // A full / empty, B full / empty
-    static constexpr int STATS_BYTES = 8 * N_TILE * 8;           // [8 consumer warps][N_TILE] float2
+    // [PARTS][N_TILE] float2 partial statistics: the 8 consumer warps of a pixel-major tile, the 2 warpgroups of an N = 64
+    // tile; N = 128 tiles share nothing
+    static constexpr int STATS_PARTS = N_TILE < SWAP_N_TILE ? 8 : N_TILE == SWAP_N_TILE ? 2 : 0;
+    static constexpr int STATS_BYTES = STATS_PARTS * N_TILE * 8;
     static constexpr int SMEM_BYTES = 1024 + RING_BYTES + BAR_BYTES + STATS_BYTES;
     static_assert(B_STAGE_BYTES % 1024 == 0, "B entries must keep the 1024-byte swizzle alignment");
     static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the shared memory of a block");
@@ -253,9 +261,9 @@ __device__ __forceinline__ void warp_tile_stats(const float* acc, bool v0, bool 
     }
 }
 
-// s_stats of the PARTS partial rows (8 consumer warps, or 2 warpgroups when swapped) -> one f64 atomic pair per column
-// of the tile (all consumer threads).
-template <int N_TILE, int PARTS = 8>
+// s_stats of the PARTS partial rows (8 consumer warps, or 2 warpgroups of an N = 64 tile) -> one f64 atomic pair per
+// column of the tile (all consumer threads).
+template <int N_TILE, int PARTS>
 __device__ __forceinline__ void flush_tile_stats(const ConvParams& P, const float2* s_stats, int img, int n_idx)
 {
     consumer_sync();
@@ -272,7 +280,7 @@ __device__ __forceinline__ void flush_tile_stats(const ConvParams& P, const floa
     consumer_sync();
 }
 
-// Plain epilogue: accumulators -> fp32 NHWC global + InstanceNorm partial statistics.
+// Pixel-major epilogue (N tiles of 16 / 32): accumulators -> fp32 NHWC global + InstanceNorm partial statistics.
 template <int N_TILE>
 __device__ __forceinline__ void epilogue_plain(const ConvParams& P, float* acc, const TileCoord& t, int warp, unsigned lane,
                                                float2* s_stats)
@@ -306,29 +314,41 @@ __device__ __forceinline__ void epilogue_plain(const ConvParams& P, float* acc, 
     }
     if (P.stats) {
         warp_tile_stats<N_TILE>(acc, valid[0], valid[1], warp, lane, s_stats);
-        flush_tile_stats<N_TILE>(P, s_stats, t.img, t.n_idx);
+        flush_tile_stats<N_TILE, 8>(P, s_stats, t.img, t.n_idx);
     }
 }
 
-// Epilogue of the swapped orientation: the accumulator is D^T, d[4j + 2h + e] = channel 16(warp%4) + lane/4 + 8h of the
-// N tile at pixel (tile row 16(warp/4) + j, column 2(lane%4) + e).  fp32 NHWC stores: one warp-wide store covers
-// 4 pixels x 8 consecutive channels, whole 32-byte sectors.  Channel statistics: in-thread over the valid pixels, the
-// quad (lanes of one channel) by shuffles, the two warpgroups through s_stats.
-__device__ __forceinline__ void epilogue_swapped(const ConvParams& P, float* acc, const TileCoord& t, int warp, unsigned lane,
-                                                 float2* s_stats)
+// Epilogue of the channel-major orientation: the accumulator is D^T, d[4j + 2h + e] = channel c0 + 8h of the N tile at
+// pixel (tile row row0 + j, column 2(lane%4) + e), c0 = c_base + 16(warp%4) + lane/4, where warpgroup g has c_base =
+// 64 g, row0 = 0 for N tiles of 128 and c_base = 0, row0 = 16 g for N tiles of 64.  fp32 NHWC stores: one warp-wide store
+// covers 4 pixels x 8 consecutive channels, whole 32-byte sectors.  Each thread's two channels are complete in the warp:
+// in-thread sums over the valid pixels, then two quad shuffles.  N = 128: the quad leader issues the f64 atomics, with no
+// shared memory and no barrier, so the two warpgroups never wait for each other.  N = 64: both warpgroups hold the same
+// channels, and the two halves meet in s_stats before one atomic pair per channel and tile: with an atomic pair per
+// warpgroup (twice the same-address f64 atomics on an image's 64 channels) the stem and the 64+64->64 skipper ran
+// 4-22 % slower (DESIGN section 5).  In a merged transposed plan N column col is channel col % phase_cols of
+// sub-pixel phase ph = col / phase_cols, written to output pixel (2y + (ph >> 1), 2x + (ph & 1)).
+template <int N_TILE>
+__device__ __forceinline__ void epilogue_channel_major(const ConvParams& P, float* acc, const TileCoord& t, int warp,
+                                                       unsigned lane, float2* s_stats)
 {
-    constexpr int N = SWAP_N_TILE;
     const int wg = warp >> 2;
-    const int c0 = 16 * (warp & 3) + (int)(lane >> 2);                // channels c0 and c0 + 8 of the N tile
-    const int y0 = t.y0 + 16 * wg, x0 = t.x0 + 2 * (int)(lane & 3);
+    const int c_base = N_TILE == MAX_N_TILE ? 64 * wg : 0, row0 = N_TILE == MAX_N_TILE ? 0 : 16 * wg;
+    const int c0 = c_base + 16 * (warp & 3) + (int)(lane >> 2);       // channels c0 and c0 + 8 of the N tile
+    const int y0 = t.y0 + row0, x0 = t.x0 + 2 * (int)(lane & 3);
     const int rows = P.dom_h - y0;                                     // row j is in the domain iff j < rows
     const bool vx[2] = {x0 < P.dom_w, x0 + 1 < P.dom_w};
+    // output channel of c0 and its offset from the pixel's NHWC address; phase_cols is a multiple of 32, so channel
+    // c0 + 8 is in the same phase at ch + 8
+    const int col = t.n_idx * N_TILE + c0;
+    const int ph = P.phase_cols > 0 ? col / P.phase_cols : 0;
+    const int ch = col - ph * P.phase_cols;
+    const size_t coff = ((size_t)(ph >> 1) * P.out_w + (ph & 1)) * P.cout + ch;
     if (P.out_scale != 1.f) {
 #pragma unroll
         for (int i = 0; i < 64; i++) acc[i] *= P.out_scale;
     }
     if (P.out) {
-        float* obase = P.out + (size_t)t.n_idx * N + c0;
 #pragma unroll
         for (int j = 0; j < 16; j++) {
             if (j >= rows) break;
@@ -336,9 +356,9 @@ __device__ __forceinline__ void epilogue_swapped(const ConvParams& P, float* acc
 #pragma unroll
             for (int e = 0; e < 2; e++) {
                 if (!vx[e]) continue;
-                float* o = obase + (orow + (P.ox_mul * (x0 + e) + P.ox_add)) * P.cout;
-                o[0] = acc[4 * j + e];
-                o[8] = acc[4 * j + 2 + e];
+                float* o = P.out + (orow + (P.ox_mul * (x0 + e) + P.ox_add)) * P.cout;
+                o[coff] = acc[4 * j + e];
+                o[coff + 8] = acc[4 * j + 2 + e];
             }
         }
     }
@@ -364,11 +384,20 @@ __device__ __forceinline__ void epilogue_swapped(const ConvParams& P, float* acc
                 q[h] += __shfl_xor_sync(0xffffffffu, q[h], off);
             }
         }
-        if ((lane & 3) == 0) {
-            s_stats[wg * N + c0] = make_float2(s[0], q[0]);
-            s_stats[wg * N + c0 + 8] = make_float2(s[1], q[1]);
+        if constexpr (N_TILE == SWAP_N_TILE) {
+            if ((lane & 3) == 0) {
+                s_stats[wg * N_TILE + c0] = make_float2(s[0], q[0]);
+                s_stats[wg * N_TILE + c0 + 8] = make_float2(s[1], q[1]);
+            }
+            flush_tile_stats<N_TILE, 2>(P, s_stats, t.img, t.n_idx);
+        } else if ((lane & 3) == 0) {
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                double* dst = P.stats + 2 * ((size_t)t.img * P.cout + ch + 8 * h);
+                atomicAdd(dst, (double)s[h]);
+                atomicAdd(dst + 1, (double)q[h]);
+            }
         }
-        flush_tile_stats<N, 2>(P, s_stats, t.img, t.n_idx);
     }
 }
 
@@ -393,28 +422,28 @@ struct Regs {
     static_assert(PRODUCER >= 40 && PRODUCER % 8 == 0 && CONSUMER % 8 == 0, "setmaxnreg takes multiples of 8");
 };
 
-// One fp16 wgmma step of the tile: activation rows x weight rows, or (SWAP) weight rows x activation rows on 128 pixels.
-template <int N_TILE, bool SWAP>
+// One fp16 wgmma step of the tile: activation rows x weight rows, or (CM) 64 weight rows x activation rows on 128 pixels.
+template <int N_TILE, bool CM>
 __device__ __forceinline__ void mma_f16(float* d, uint64_t act, uint64_t w) {
-    if constexpr (SWAP) wgmma_f16<128>(d, w, act);
-    else                wgmma_f16<N_TILE>(d, act, w);
+    if constexpr (CM) wgmma_f16<128>(d, w, act);
+    else              wgmma_f16<N_TILE>(d, act, w);
 }
-template <int N_TILE, bool SWAP>
+template <int N_TILE, bool CM>
 __device__ __forceinline__ void mma_e4m3(float* d, uint64_t act, uint64_t w) {
-    if constexpr (SWAP) wgmma_e4m3<128>(d, w, act);
-    else                wgmma_e4m3<N_TILE>(d, act, w);
+    if constexpr (CM) wgmma_e4m3<128>(d, w, act);
+    else              wgmma_e4m3<N_TILE>(d, act, w);
 }
 
 template <int N_TILE, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1) __maxnreg__((Regs<N_TILE, MODE>::LAUNCH))
 k_conv_wg(const __grid_constant__ ConvParams P)
 {
-    // N tile 64 always runs the swapped orientation (256-pixel tiles, see the top of the file); plan creation sized its
-    // tiles and boxes with tile_rows(n_tile) to match.
-    constexpr bool SWAP = N_TILE == SWAP_N_TILE;
+    // N tiles of 64 and 128 run channel-major (N = 64 on 256-pixel tiles, see the top of the file); plan creation sized
+    // its tiles and boxes with tile_rows(n_tile) to match.
+    constexpr bool CM = N_TILE >= SWAP_N_TILE;
     constexpr bool SPLIT = MODE != MODE_FP16;
-    constexpr int TH = SWAP ? SWAP_TILE_H : TILE_H;                  // tile rows; each consumer warpgroup owns half
-    constexpr int ACC = SWAP ? 64 : N_TILE / 2;                       // fp32 accumulators per consumer thread
+    constexpr int TH = N_TILE == SWAP_N_TILE ? SWAP_TILE_H : TILE_H;  // tile rows
+    constexpr int ACC = CM ? 64 : N_TILE / 2;                         // fp32 accumulators per consumer thread
     using C = Cfg<N_TILE, SPLIT>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -425,7 +454,7 @@ k_conv_wg(const __grid_constant__ ConvParams P)
     uint64_t* a_empty = a_full + MAX_STAGES;
     uint64_t* b_full = a_empty + MAX_STAGES;
     uint64_t* b_empty = b_full + MAX_STAGES;
-    float2* s_stats = reinterpret_cast<float2*>(smem + RING_BYTES + C::BAR_BYTES);   // [8][N_TILE]
+    float2* s_stats = reinterpret_cast<float2*>(smem + RING_BYTES + C::BAR_BYTES);   // [Cfg::STATS_PARTS][N_TILE]
 
     const int warp = threadIdx.x >> 5;
     const unsigned lane = threadIdx.x & 31;
@@ -495,11 +524,14 @@ k_conv_wg(const __grid_constant__ ConvParams P)
             }
         }
     } else {
-        // ================================ consumers (2 warpgroups, half of the tile rows each) ========
+        // ================================ consumers (2 warpgroups) =====================================
         asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(Regs<N_TILE, MODE>::CONSUMER));
-        const uint32_t smem_base = smem_u32(smem);
-        const uint32_t b_base = smem_u32(b_ring);
-        const uint32_t a_row0 = (uint32_t)(warp >> 2) * (TH / 2) * ROW_BYTES;   // tile rows (TH/2) g .. (TH/2)(g + 1) - 1
+        // Warpgroup g reads weight rows 64 g .. 64 g + 63 on all 16 tile rows (N tile 128), or all weight rows on tile
+        // rows (TH/2) g .. (TH/2)(g + 1) - 1 (N tiles of 16 .. 64).
+        constexpr bool CH_SPLIT = N_TILE == MAX_N_TILE;
+        const uint32_t wg = (uint32_t)(warp >> 2);
+        const uint32_t a_base = smem_u32(smem) + (CH_SPLIT ? 0 : wg * (TH / 2) * ROW_BYTES);
+        const uint32_t b_base = smem_u32(b_ring) + (CH_SPLIT ? wg * 64 * 128 : 0);
         // The e4m3 products get their own accumulator: Hopper's fp8 wgmma adds into D with a reduced-precision
         // accumulation, which would truncate the fp16 main product's fp32 sum.  The two are added in the epilogue.
         float acc[ACC];
@@ -518,21 +550,21 @@ k_conv_wg(const __grid_constant__ ConvParams P)
                 const int cnt = P.g_cnt[g];
                 for (int chunk = 0; chunk < nchunks; chunk++) {
                     mbar_wait(a_full + as, aph);
-                    const uint32_t a_hi = smem_base + as * a_stage_bytes + a_row0;
+                    const uint32_t a_hi = a_base + as * a_stage_bytes;
                     for (int i = 0; i < cnt; i++) {
                         mbar_wait(b_full + bs, bph);
-                        const uint32_t ai = a_hi + i * ROW_BYTES, al = ai + a_op_bytes;      // tap i: rows i .. i + TH/2 - 1
+                        const uint32_t ai = a_hi + i * ROW_BYTES, al = ai + a_op_bytes;      // tap i: i box rows further in
                         const uint32_t b_hi = b_base + bs * C::B_STAGE_BYTES, b_lo = b_hi + C::B_BYTES;
                         wgmma_fence();
 #pragma unroll
                         for (int k = 0; k < KCHUNK / 16; k++) {
                             const uint64_t da = make_desc(ai + k * 32), db = make_desc(b_hi + k * 32);
-                            mma_f16<N_TILE, SWAP>(acc, da, db);
+                            mma_f16<N_TILE, CM>(acc, da, db);
                             if constexpr (MODE == MODE_F8) {
-                                mma_e4m3<N_TILE, SWAP>(acc8, make_desc(al + k * 32), make_desc(b_lo + k * 32));
+                                mma_e4m3<N_TILE, CM>(acc8, make_desc(al + k * 32), make_desc(b_lo + k * 32));
                             } else if constexpr (MODE == MODE_FP16X3) {
-                                mma_f16<N_TILE, SWAP>(acc, da, make_desc(b_lo + k * 32));
-                                mma_f16<N_TILE, SWAP>(acc, make_desc(al + k * 32), db);
+                                mma_f16<N_TILE, CM>(acc, da, make_desc(b_lo + k * 32));
+                                mma_f16<N_TILE, CM>(acc, make_desc(al + k * 32), db);
                             }
                         }
                         wgmma_commit();
@@ -560,8 +592,8 @@ k_conv_wg(const __grid_constant__ ConvParams P)
                 for (int i = 0; i < ACC; i++) { acc_fence(acc8[i]); acc[i] += acc8[i]; }
             }
             if (lane == 0) { mbar_arrive(b_empty + prev_b); mbar_arrive(a_empty + prev_a); }
-            if constexpr (SWAP) epilogue_swapped(P, acc, t, warp, lane, s_stats);
-            else                epilogue_plain<N_TILE>(P, acc, t, warp, lane, s_stats);
+            if constexpr (CM) epilogue_channel_major<N_TILE>(P, acc, t, warp, lane, s_stats);
+            else              epilogue_plain<N_TILE>(P, acc, t, warp, lane, s_stats);
         }
     }
 }
@@ -861,7 +893,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
             // Merged transposed conv: ONE stride-1 pass over the input grid with the four taps (dy, dx) in {0,1}^2 and
             // N = 4 x cout columns = the four sub-pixel phases (weights from the host in [tap][phase*cout + co][cin] layout,
             // zero where a phase does not use a tap: 9 of 16 blocks are non-zero).  One launch, one read of every input tile.
-            s.n_tile = MAX_N_TILE;                            // the swapped N = 64 epilogue has no phase columns
+            s.n_tile = MAX_N_TILE;
             s.ncols = 4 * d->cout;
             LWB_CHECK_ARG(d->cout % 32 == 0 && s.ncols % s.n_tile == 0, "merged transposed conv needs cout in multiples of 32");
             for (int t = 0; t < 4; t++) s.tap(t >> 1, t & 1, 0, t);

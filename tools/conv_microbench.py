@@ -8,16 +8,32 @@ operand bytes per algorithmic FLOP that the TMA unit moves from L2 into shared m
 engine runs ("run"): the same 16 x 8 tiles for N tiles of 16..128, the swapped 32 x 8 tiles for an N tile of 64.
 
     python tools/conv_microbench.py [--batch 8] [--reps 50] [--only res] [--json out.json]
+
+``--compare A B`` times the builds of two source trees (each a checkout with its library built) against each other:
+one worker process per tree, both on the same GPU, the same layer and mode timed in both, ``--rounds`` times with the
+order alternating, and the median of each printed with their ratio B / A.
+
+    python tools/conv_microbench.py --compare ../parent . [--batch 8] [--rounds 7] [--json cmp.json]
 """
 import argparse
 import json
+import os
+import statistics
+import subprocess
 import sys
 
 import torch
 
-sys.path.insert(0, ".")
-from impersonator_b200 import kernels as K  # noqa: E402
-from impersonator_b200.generator import merge_transposed_weight  # noqa: E402
+K = merge_transposed_weight = None
+
+
+def load(tree):
+    """Imports the conv engine of the source tree at `tree`."""
+    global K, merge_transposed_weight
+    sys.path.insert(0, os.path.abspath(tree))
+    from impersonator_b200 import kernels
+    from impersonator_b200.generator import merge_transposed_weight as mtw
+    K, merge_transposed_weight = kernels, mtw
 
 TILE_H, TILE_W, KCHUNK, MAX_GROUP = 16, 8, 64, 8
 SWAP_N_TILE, SWAP_TILE_H = 64, 32            # N = 64 plans run 64 channels x (32 x 8) pixels
@@ -161,13 +177,70 @@ def time_plan(plan, reps):
     return e0.elapsed_time(e1) / reps
 
 
+def worker(tree, batch, reps):
+    """--compare worker: one request per line on stdin, "<layer index> <split>", answered with the time in ms."""
+    load(tree)
+    dev = torch.device("cuda")
+    torch.set_grad_enabled(False)
+    for req in sys.stdin:
+        li, split = map(int, req.split())
+        torch.manual_seed(0)
+        plan, _ = make_plan(LAYERS[li][1], batch, split, dev)
+        print(repr(time_plan(plan, reps)), flush=True)
+        del plan
+
+
+def compare(a):
+    trees = a.compare
+    cmd = [sys.executable, os.path.abspath(__file__), "--batch", str(a.batch), "--reps", str(a.reps), "--worker"]
+    procs = [subprocess.Popen(cmd + [t], stdin=subprocess.PIPE, stdout=subprocess.PIPE, text=True) for t in trees]
+
+    def ask(p, li, split):
+        p.stdin.write("%d %d\n" % (li, split))
+        p.stdin.flush()
+        return float(p.stdout.readline())
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    print("A = %s, B = %s; %s; batch %d, %d rounds x %d reps" % (trees[0], trees[1], gpu, a.batch, a.rounds, a.reps))
+    print("%-34s %-7s %9s %9s %7s" % ("layer", "mode", "A ms", "B ms", "B / A"))
+    rows = []
+    for li, (name, _) in enumerate(LAYERS):
+        if a.only and a.only not in name:
+            continue
+        for mode, split in MODES:
+            ms = ([], [])
+            for r in range(a.rounds):
+                for i in ((0, 1) if r % 2 == 0 else (1, 0)):
+                    ms[i].append(ask(procs[i], li, split))
+            med = [statistics.median(m) for m in ms]
+            rows.append(dict(layer=name, mode=mode, a_ms=med[0], b_ms=med[1], ratio=med[1] / med[0], a_all=ms[0], b_all=ms[1]))
+            print("%-34s %-7s %9.4f %9.4f %7.3f" % (name, mode, med[0], med[1], med[1] / med[0]), flush=True)
+    for p in procs:
+        p.stdin.close()
+        p.wait()
+    tot = [sum(r[k] for r in rows if r["mode"] == "fp16f8") for k in ("a_ms", "b_ms")]
+    print("fp16f8 total: A %.4f ms, B %.4f ms, B / A %.3f" % (tot[0], tot[1], tot[1] / tot[0]))
+    if a.json:
+        with open(a.json, "w") as f:
+            json.dump(dict(gpu=gpu, a=trees[0], b=trees[1], batch=a.batch, reps=a.reps, rounds=a.rounds, rows=rows), f, indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--only", default="", help="substring filter on the layer name")
     ap.add_argument("--json", default="", help="also write the rows to this file")
+    ap.add_argument("--compare", nargs=2, metavar=("A", "B"), help="time the builds of two source trees against each other")
+    ap.add_argument("--rounds", type=int, default=7, help="--compare: timings per layer, mode and tree")
+    ap.add_argument("--worker", help=argparse.SUPPRESS)
     a = ap.parse_args()
+    if a.worker:
+        return worker(a.worker, a.batch, a.reps)
+    if a.compare:
+        return compare(a)
+    load(".")
     dev = torch.device("cuda")
     torch.manual_seed(0)
     torch.set_grad_enabled(False)
