@@ -49,18 +49,33 @@ class Operands(object):
         return dict(y_f32=self.f32, y_hi=self.hi, y_lo=self.lo)
 
 
-def pack_all(items, split):
-    """[(weight, transposed, cout_pad, cin_pad)] -> [PackedWeight]: max|w| of every layer is read back in ONE host sync
-    (it sets the per-layer weight exponent, kernels.weight_exponent), then each layer is packed."""
-    amax = torch.stack([w.abs().max().float() for w, _, _, _ in items]).tolist()
-    return [K.pack_conv_weight(w, transposed=t, cout_pad=co, cin_pad=ci, split=split, absmax=a)
-            for (w, t, co, ci), a in zip(items, amax)]
+def _convt_merge():
+    """LWB_CONVT_MERGE (default 1): ConvTranspose2d(k3, s2, p1, op1) layers with up to 128 output channels run as ONE
+    stride-1 pass with the four sub-pixel phases stacked on N (merge_transposed_weight) instead of four phase launches."""
+    return os.environ.get("LWB_CONVT_MERGE", "1") != "0"
+
+
+def merge_transposed_weight(wt):
+    """IOHW [cin, cout, 3, 3] of ConvTranspose2d(k=3, s=2, p=1, output_padding=1) -> OIHW [4*cout, cin, 2, 2]: output
+    channel block ph = 2a + b holds sub-pixel phase out[2y+a, 2x+b]; filter tap (dy, dx) reads in[y+dy, x+dx].
+    Per axis: phase 0 uses k=1 at d=0; phase 1 uses k=2 at d=0 and k=0 at d=1 (oy = 2*iy - 1 + ky); the other 7 of the 16
+    (phase, tap) blocks are zero."""
+    cin, cout = wt.shape[0], wt.shape[1]
+    k_of = ({0: 1}, {0: 2, 1: 0})
+    out = torch.zeros((4 * cout, cin, 2, 2), dtype=torch.float32, device=wt.device)
+    for a in range(2):
+        for b in range(2):
+            ph = 2 * a + b
+            for dy, ky in k_of[a].items():
+                for dx, kx in k_of[b].items():
+                    out[ph * cout:(ph + 1) * cout, :, dy, dx] = wt[:, :, ky, kx].t().float()
+    return out
 
 
 class Conv(object):
     """One convolution bound to its operands: ``desc``, the raw fp32 NHWC output ``out`` and, after
     PlanBinder.finalize(), ``plan``."""
-    __slots__ = ("desc", "x", "weight", "cout_pad", "cin_pad", "out", "plan")
+    __slots__ = ("desc", "x", "x1", "weight", "cout_pad", "cin_pad", "stats", "out", "plan")
 
 
 class PlanBinder(object):
@@ -72,31 +87,50 @@ class PlanBinder(object):
         self._convs = []
 
     def conv(self, weight, x, n, h, w, stride=1, pad=None, pad_w=None, dil=1, cout_pad=None, cin_pad=None, out=None,
-             share=None):
+             share=None, x1=None, transposed=False, rowk=False, row_pitch=0, n_tile=0, halo=False, split=None,
+             stats=None):
         """weight OIHW fp32 over operands x = (hi, lo) of [n, h, w, cin_pad or cin]; pad defaults to kh // 2.  The raw
         output [n, ho, wo, cout_pad or cout] is ``out`` when given, else the buffer shared by every conv of this binder
-        with the same output shape and ``share`` tag when one is given, else a buffer of its own."""
-        cout, cin, kh, kw = weight.shape
+        with the same output shape and ``share`` tag when one is given, else a buffer of its own.
+        x1: second operand pair of a concat input, its channels follow those of x.  transposed: IOHW weights of a
+        ConvTranspose2d(k3, s2, p1, op1), run as one merged-phase pass (lwb_conv_desc.transposed = 2) where
+        LWB_CONVT_MERGE and the shape allow.  rowk: the 7x7 row-K stem over rows of ``row_pitch`` pixels of cin_pad
+        channels.  n_tile / halo: lwb_conv_desc's forced N tile and halo variant.  split: this conv's operand mode (the
+        binder's by default).  stats: f64 [n, cout, 2] InstanceNorm sums the plan accumulates."""
+        cout, cin = (weight.shape[1], weight.shape[0]) if transposed else (weight.shape[0], weight.shape[1])
+        kh, kw = weight.shape[2:]
+        cin1 = x1[0].shape[3] if x1 is not None else 0
         r = Conv()
-        r.desc = K.make_conv_desc(n, h, w, cin_pad or cin, cout_pad or cout, kh, kw, stride=stride,
-                                  pad=kh // 2 if pad is None else pad, pad_w=pad_w, dil=dil, split=self.split)
+        r.desc = K.make_conv_desc(n, h, w, (cin_pad or cin) - cin1, cout_pad or cout, kh, kw, stride=stride,
+                                  pad=kh // 2 if pad is None else pad, pad_w=pad_w, dil=dil, cin1=cin1,
+                                  transposed=transposed, split=self.split if split is None else split, rowk=rowk,
+                                  row_pitch=row_pitch, n_tile=n_tile, halo=halo)
+        if transposed and _convt_merge() and cout <= 128 and cout % 32 == 0 and (kh, kw) == (3, 3):
+            r.desc.transposed = 2
+            weight = merge_transposed_weight(weight)
         shape = (n, r.desc.h_out, r.desc.w_out, cout_pad or cout)
         if out is None and share is not None:
             out = self._shared.get((shape, share))
             if out is None:
                 out = self._shared[(shape, share)] = torch.empty(shape, dtype=torch.float32, device=self.dev)
         r.out = out if out is not None else torch.empty(shape, dtype=torch.float32, device=self.dev)
-        r.x, r.weight, r.cout_pad, r.cin_pad, r.plan = x, weight, cout_pad, cin_pad, None
+        r.x, r.x1, r.weight, r.cout_pad, r.cin_pad, r.stats, r.plan = x, x1, weight, cout_pad, cin_pad, stats, None
         self._convs.append(r)
         return r
 
     def finalize(self):
-        """Pack the weights and create every K.ConvPlan; the fp32 source weights are released."""
-        packed = pack_all([(r.weight, False, r.cout_pad, r.cin_pad) for r in self._convs], self.split)
-        for r, wp in zip(self._convs, packed):
-            r.plan = K.ConvPlan(r.desc, r.x, None, wp, r.out, None)
+        """Pack the weights and create every K.ConvPlan; the fp32 source weights are released.  max|w| of every layer
+        is read back in ONE host sync (it sets the per-layer weight exponent, kernels.weight_exponent)."""
+        convs, self._convs = self._convs, []
+        amax = torch.stack([r.weight.abs().max().float() for r in convs]).tolist()
+        packed = [K.pack_conv_weight_rowk(r.weight, cout_pad=r.cout_pad, cpx=r.cin_pad, split=r.desc.split, absmax=a)
+                  if r.desc.rowk else
+                  K.pack_conv_weight(r.weight, transposed=r.desc.transposed == 1, cout_pad=r.cout_pad, cin_pad=r.cin_pad,
+                                     split=r.desc.split, absmax=a)
+                  for r, a in zip(convs, amax)]
+        for r, wp in zip(convs, packed):
+            r.plan = K.ConvPlan(r.desc, r.x, r.x1, wp, r.out, r.stats)
             r.weight = None
-        self._convs = []
 
 
 def stream_for(owner, cls, key, *args, limit, **kw):

@@ -13,7 +13,7 @@ reference, so checkpoints (``BaseModel._load_params``, models/models.py:159-179)
 
 The ``nn.Conv2d`` / ``nn.InstanceNorm2d`` / ``nn.ConvTranspose2d`` children are parameter holders
 only (they give the reference's key names and default init); every forward path goes through
-``_UnetStream`` / ``_ResnetStream`` below, which drive hand-written sm_90a kernels:
+``_Stream`` below, which drive hand-written sm_90a kernels:
 wgmma implicit-GEMM convs (fp16 hi/lo split operands, fp32 accumulate), a fused
 InstanceNorm+ReLU+residual+Liquid-Warping-Block kernel, and the 7x7 heads.  There is no torch
 fallback: without the CUDA library the calls raise.
@@ -31,7 +31,8 @@ import torch.nn as nn
 
 from . import kernels as K
 from ._lib import LwbError
-from .binding import Operands, StreamOwner, pack_all, precision_mode, split_mode, stream_for
+from .binding import Operands, PlanBinder, StreamOwner, precision_mode, split_mode, stream_for
+from .binding import merge_transposed_weight  # noqa: F401  (callers import it from the generator too)
 
 
 _WEIGHTS_EPOCH = [0]
@@ -70,39 +71,12 @@ def _tc_heads():
     return os.environ.get("LWB_TC_HEADS", "1") != "0"
 
 
-def _convt_merge():
-    """LWB_CONVT_MERGE (default 1): ConvTranspose2d(k3, s2, p1, op1) layers with up to 128 output channels run as ONE
-    stride-1 pass with the four sub-pixel phases stacked on N (merge_transposed_weight) instead of four phase launches."""
-    return os.environ.get("LWB_CONVT_MERGE", "1") != "0"
-
-
-def merge_transposed_weight(wt):
-    """IOHW [cin, cout, 3, 3] of ConvTranspose2d(k=3, s=2, p=1, output_padding=1) -> OIHW [4*cout, cin, 2, 2]: output
-    channel block ph = 2a + b holds sub-pixel phase out[2y+a, 2x+b]; filter tap (dy, dx) reads in[y+dy, x+dx].
-    Per axis: phase 0 uses k=1 at d=0; phase 1 uses k=2 at d=0 and k=0 at d=1 (oy = 2*iy - 1 + ky); the other 7 of the 16
-    (phase, tap) blocks are zero."""
-    cin, cout = wt.shape[0], wt.shape[1]
-    k_of = ({0: 1}, {0: 2, 1: 0})
-    out = torch.zeros((4 * cout, cin, 2, 2), dtype=torch.float32, device=wt.device)
-    for a in range(2):
-        for b in range(2):
-            ph = 2 * a + b
-            for dy, ky in k_of[a].items():
-                for dx, kx in k_of[b].items():
-                    out[ph * cout:(ph + 1) * cout, :, dy, dx] = wt[:, :, ky, kx].t().float()
-    return out
-
-
 def fold_head_weights(w_img, w_att):
     """[3,64,7,7] + [1,64,7,7] -> [32, 64, 7, 1]: output channel kx*4 + co of the (7 x 1) filter = column kx of head co
     (networks/generator.py:126-134; rows 28..31 are zero)."""
     w4 = torch.cat([w_img, w_att], dim=0).float()                      # [4, C, ky, kx]
     folded = w4.permute(3, 0, 1, 2).reshape(28, w4.shape[1], 7, 1)     # [kx*4+co, C, ky, 1]
     return torch.cat([folded, torch.zeros(4, w4.shape[1], 7, 1, dtype=folded.dtype, device=folded.device)], dim=0).contiguous()
-
-
-def _align_corners():
-    return K.default_align_corners()
 
 
 def _halo_mode():
@@ -211,175 +185,122 @@ class ResidualBlock(nn.Module):
 # ------------------------------------------------------------------------------------------
 # engine: one network bound to (batch, H, W, precision) -> persistent buffers + conv plans
 # ------------------------------------------------------------------------------------------
-class _Layer(object):
-    """conv (+ InstanceNorm params) bound to buffers: plan + stats slot."""
-    __slots__ = ("plan", "raw", "stats", "gamma", "beta", "w", "wsrc")
+class _Stream(object):
+    """ResUnetGenerator (networks/generator.py:68-184) or ResNetGenerator (networks/generator.py:23-65, the BG net: the
+    same chain without skippers and warps) bound to fixed shapes."""
 
-
-class _StreamBase(object):
-    def __init__(self, B, H, W, dev, split):
-        self.B, self.H, self.W, self.dev, self.split = B, H, W, dev, split
-        self._stats_slots = []
-        self._layers = []
-        self._raw = {}
-        self.ws = None
-
-    def _raw_buf(self, h, w, c):
-        key = (h, w, c)
-        if key not in self._raw:
-            self._raw[key] = torch.empty((self.B, h, w, c), dtype=torch.float32, device=self.dev)
-        return self._raw[key]
-
-    def _make_layer(self, conv, norm, x0, x1=None, stride=1, transposed=False, rowk=False, row_pitch=0, h=None, w=None,
-                    halo=False, weight=None, pad=None, n_tile=0, pad_w=None):
-        L = _Layer()
-        wt = (weight if weight is not None else conv.weight).detach()
-        L.wsrc = None
-        if rowk:
-            L.w = K.pack_conv_weight_rowk(wt, split=min(self.split, 1))       # the stem keeps the fp16 hi/lo input
-            cout, kh, kw = wt.shape[0], wt.shape[2], wt.shape[3]
-            d = K.make_conv_desc(self.B, h, w, 8, cout, kh, kw, stride=1, pad=kh // 2, split=min(self.split, 1),
-                                 rowk=True, row_pitch=row_pitch, halo=halo)
-        else:
-            L.w = None
-            cout = wt.shape[1] if transposed else wt.shape[0]
-            kh, kw = wt.shape[2], wt.shape[3]
-            merged = bool(transposed and _convt_merge() and cout <= 128 and cout % 32 == 0 and (kh, kw) == (3, 3))
-            # packed in _finalize (one max|w| sync for the whole stream)
-            L.wsrc = (merge_transposed_weight(wt), False) if merged else (wt, transposed)
-            cin0 = x0[0].shape[3]
-            cin1 = x1[0].shape[3] if x1 is not None else 0
-            d = K.make_conv_desc(self.B, h, w, cin0, cout, kh, kw, stride=stride,
-                                 pad=(pad if pad is not None else conv.padding[0]),
-                                 cin1=cin1, transposed=transposed, split=self.split, halo=halo, n_tile=n_tile, pad_w=pad_w)
-            if merged:
-                d.transposed = 2                        # lwb_conv_desc: merged-phase weights
-        L.raw = self._raw_buf(d.h_out, d.w_out, cout)
-        L.stats = (len(self._stats_slots), cout)
-        self._stats_slots.append(cout)
-        L.gamma = norm.weight.detach().float().contiguous() if norm is not None else None
-        L.beta = norm.bias.detach().float().contiguous() if norm is not None else None
-        L.plan = (d, x0, x1)
-        self._layers.append(L)
-        return L
-
-    def _finalize(self):
-        cmax = max(max(self._stats_slots), 16)
-        # InstanceNorm statistics of every layer + the operand-range flag share one buffer: one fill per pass
-        nstat = len(self._stats_slots) * self.B * cmax * 2
-        self._zero = torch.zeros(nstat * 8 + 4, dtype=torch.uint8, device=self.dev)
-        self.stats = self._zero[:nstat * 8].view(torch.float64).view(len(self._stats_slots), self.B, cmax, 2)
+    def __init__(self, net, B, H, W, dev, split, keep_f32=False):
+        self.B, self.H, self.W, self.split = B, H, W, split
+        if isinstance(net, ResUnetGenerator):
+            enc, dec, skip = ([(s[0], s[1]) for s in seq] for seq in (net.encoders, net.decoders, net.skippers))
+            blocks = [b.main for b in net.resnets]
+            w_img, w_att = net.img_reg[0].weight.detach(), net.attetion_reg[0].weight.detach()
+        else:                                                     # the BG net: one flat Sequential, a 3-channel head
+            m, r = list(net.model), 3 * (net._n_down + 1)
+            enc = [(m[i], m[i + 1]) for i in range(0, r, 3)]
+            blocks = [b.main for b in m[r:r + net._repeat_num]]
+            dec = [(m[i], m[i + 1]) for i in range(r + net._repeat_num, len(m) - 2, 3)]
+            skip = []
+            w_img = m[-2].weight.detach()
+            w_att = torch.zeros_like(w_img[:1])
+        self.n_down = nd = len(dec)
+        if H % (1 << nd) or W % (1 << nd):
+            raise LwbError("image size must be divisible by %d" % (1 << nd))
+        self.cin = enc[0][0].weight.shape[1]
+        if self.cin > 8:
+            raise LwbError("stem supports at most 8 input channels")
+        # InstanceNorm statistics of every conv + the operand-range flag share one buffer: one fill per pass
+        norms = [m for m in net.modules() if isinstance(m, nn.InstanceNorm2d)]
+        cmax = max([16] + [m.num_features for m in norms])
+        nstat = len(norms) * B * cmax * 2
+        self._zero = torch.zeros(nstat * 8 + 4, dtype=torch.uint8, device=dev)
+        slots = iter(self._zero[:nstat * 8].view(torch.float64).view(len(norms), -1))
         self.range_flag = self._zero[nstat * 8:].view(torch.int32)
-        self.ws = torch.empty((self.B, cmax, 2), dtype=torch.float32, device=self.dev)
-        pend = [L for L in self._layers if L.wsrc is not None]
-        packed = pack_all([(L.wsrc[0], L.wsrc[1], None, None) for L in pend], self.split)
-        for L, wp in zip(pend, packed):
-            L.w, L.wsrc = wp, None
-        for L in self._layers:
-            slot, cout = L.stats
-            # per-layer contiguous [B, cout, 2] view at the head of the slot (None: no norm follows)
-            L.stats = None if self._stats_slots[slot] == 0 else \
-                self.stats[slot].view(-1)[:self.B * cout * 2].view(self.B, cout, 2)
-            d, x0, x1 = L.plan
-            L.plan = K.ConvPlan(d, x0, x1, L.w, L.raw, L.stats)
+        self.ws = torch.empty((B, cmax, 2), dtype=torch.float32, device=dev)
+        plans = PlanBinder(dev, split)
 
-    def _label_heads(self):
-        """The folded heads issue N = 32 columns; their algorithmic work is the 7x7 x 64 -> 4 convolution."""
-        L = getattr(self, 'head_layer', None)
-        if L is not None and getattr(self, 'folded_kw', 7) == 7 and L.plan.desc.kw == 1:
-            L.plan.flops = 2.0 * self.B * self.H * self.W * 49 * 64 * 4
-            L.plan.label = "H7x7 64->4 @%d (7x1 filter, N = 7 cols x 4)" % self.H
-            L.plan.prof_class = "heads"
+        def conv_norm(conv, norm, x, h, w, **kw):
+            """-> (Conv, gamma, beta); the conv accumulates its statistics in the next slot (a contiguous [B, cout, 2]
+            view at its head)."""
+            c = norm.num_features
+            stats = next(slots)[:B * c * 2].view(B, c, 2)
+            return (plans.conv(conv.weight.detach(), x, B, h, w, share="raw", stats=stats, **kw),
+                    norm.weight.detach().float().contiguous(), norm.bias.detach().float().contiguous())
+
+        hm = _halo_mode() if skip else '0'                        # the BG net ignores LWB_HALO
+        c0 = enc[0][0].weight.shape[0]
+        tc = _tc_heads() and c0 == 64                            # folded heads, unless the halo heads run
+        heads_tc = hm != '0' or tc                                # the heads read fp16 operands, else fp32
+        # stem input: padded NHWC8 (3 px border top/left/bottom, 5 right) for the row-K 7x7 conv, which keeps the fp16
+        # hi/lo input
+        self.x_pad = Operands((B, H + 6, W + 8, 8), dev, split)
+        self.enc_layers = [conv_norm(*enc[0], self.x_pad.pair, H, W, rowk=True, row_pitch=W + 8, cin_pad=8,
+                                     split=min(split, 1), halo=(hm != '0'))]
+        c, h, w = c0, H, W
+        self.e = [Operands((B, h, w, c), dev, split, f32=keep_f32)]
+        for i in range(1, nd + 1):
+            self.enc_layers.append(conv_norm(*enc[i], self.e[i - 1].pair, h, w, stride=2))
+            c, h, w = c * 2, h // 2, w // 2
+            self.e.append(Operands((B, h, w, c), dev, split, f32=(keep_f32 or i == nd)))
+        # resnets (h buffer for the mid activation)
+        self.hb = Operands((B, h, w, c), dev, split)
+        self.res_layers, self.res_out = [], []
+        prev = self.e[nd]
+        for m in blocks:
+            self.res_layers.append((conv_norm(m[0], m[1], prev.pair, h, w, halo=(hm == 'all')),
+                                    conv_norm(m[3], m[4], self.hb.pair, h, w, halo=(hm == 'all'))))
+            prev = Operands((B, h, w, c), dev, split, f32=True)
+            self.res_out.append(prev)
+        # decoders, each followed by its skipper (concat input: encoder output, decoder output) where the net has them
+        self.dec_layers, self.d_up, self.d_out = [], [], []
+        for i, (conv, norm) in enumerate(dec):
+            last = (i == nd - 1)
+            out = Operands((B, h * 2, w * 2, c // 2), dev, split, f32=(last and not heads_tc), half=(not last or heads_tc))
+            up = Operands((B, h * 2, w * 2, c // 2), dev, split) if skip else out
+            ld = conv_norm(conv, norm, prev.pair, h, w, stride=2, transposed=True)
+            c, h, w = c // 2, h * 2, w * 2
+            ls = conv_norm(*skip[i], self.e[nd - 1 - i].pair, h, w, x1=up.pair, halo=(hm != '0')) if skip else None
+            self.dec_layers.append((ld, ls))
+            self.d_up.append(up)
+            self.d_out.append(out)
+            prev = out
+        # img_reg (64->3) + attetion_reg (64->1)
+        self.head, self.folded_kw = None, 0
+        if hm != '0':
+            # one 7x7 conv padded to 16 output channels on the tensor cores (halo variant, N tile 16); channels 0..3
+            # are consumed by the composite kernel
+            w16 = torch.cat([w_img, w_att, torch.zeros(12, *w_img.shape[1:], device=w_img.device, dtype=w_img.dtype)], dim=0)
+            self.head = plans.conv(w16, prev.pair, B, H, W, halo=True, n_tile=16, share="raw")
+        elif tc:
+            # a 7 x 1 filter with N = 7 columns x 4 channels (-> 32) on the tensor cores; the composite kernel adds the
+            # seven column partials of every pixel (lwb_heads_composite, folded_kw)
+            self.head = plans.conv(fold_head_weights(w_img, w_att), prev.pair, B, H, W, pad_w=0, n_tile=32, share="raw")
+            self.folded_kw = 7
+        else:
+            self.w4 = K.pack_head_weights(w_img, w_att)
+            self.head_raw = torch.empty((B, H, W, 4), dtype=torch.float32, device=dev)
+        plans.finalize()
+        if self.head is not None:
+            self.head_raw = self.head.out
+        if self.folded_kw:
+            # the folded heads issue N = 32 columns; their algorithmic work is the 7x7 x 64 -> 4 convolution
+            p = self.head.plan
+            p.flops = 2.0 * B * H * W * 49 * 64 * 4
+            p.label = "H7x7 64->4 @%d (7x1 filter, N = 7 cols x 4)" % H
+            p.prof_class = "heads"
+        self.head_flag = self.range_flag if split == 2 and skip else None     # the BG net's heads report no range bit
 
     def begin_pass(self):
         """Zero the InstanceNorm statistics and the range flag (one fill)."""
         self._zero.zero_()
         self.pass_id = _PASS[0]
 
-    def _conv_norm(self, L, out, relu, residual=None, warp_src=None, T=None, ac=False):
-        L.plan.run()
-        K.norm_act_nhwc(L.raw, L.stats, L.gamma, L.beta, relu, self.ws, residual=residual, warp_src=warp_src, T=T,
+    def _conv_norm(self, layer, out, relu, residual=None, warp_src=None, T=None, ac=False):
+        conv, gamma, beta = layer
+        conv.plan.run()
+        K.norm_act_nhwc(conv.out, conv.stats, gamma, beta, relu, self.ws, residual=residual, warp_src=warp_src, T=T,
                         align_corners=ac, y_f32=out.f32, y_hi=out.hi, y_lo=out.lo, lo_format=1 if self.split == 2 else 0,
                         range_flag=self.range_flag)
-
-
-class _UnetStream(_StreamBase):
-    """ResUnetGenerator (networks/generator.py:68-184) bound to fixed shapes."""
-
-    def __init__(self, net, B, H, W, dev, split, keep_f32=False):
-        super(_UnetStream, self).__init__(B, H, W, dev, split)
-        self.n_down, self.repeat = net.n_down, net.repeat_num
-        nd = self.n_down
-        if H % (1 << nd) or W % (1 << nd):
-            raise LwbError("image size must be divisible by %d" % (1 << nd))
-        self.keep_f32 = keep_f32
-        # stem input: padded NHWC8 (3 px border top/left/bottom, 5 right) for the row-K 7x7 conv
-        self.pitch = W + 8
-        self.x_pad = Operands((B, H + 6, self.pitch, 8), dev, split)
-        self.cin = net.encoders[0][0].weight.shape[1]
-        if self.cin > 8:
-            raise LwbError("stem supports at most 8 input channels")
-        # encoders
-        self.e, self.enc_layers = [], []
-        c, h, w = net.encoders[0][0].weight.shape[0], H, W
-        hm = _halo_mode()
-        self.enc_layers.append(self._make_layer(net.encoders[0][0], net.encoders[0][1], self.x_pad.pair, rowk=True,
-                                                row_pitch=self.pitch, h=H, w=W, halo=(hm != '0')))
-        self.e.append(Operands((B, h, w, c), dev, split, f32=keep_f32))
-        for i in range(1, nd + 1):
-            self.enc_layers.append(self._make_layer(net.encoders[i][0], net.encoders[i][1], self.e[i - 1].pair,
-                                                    stride=2, h=h, w=w))
-            c, h, w = c * 2, h // 2, w // 2
-            self.e.append(Operands((B, h, w, c), dev, split, f32=(keep_f32 or i == nd)))
-        # resnets (ping-pong x buffers; h buffer for the mid activation)
-        self.hb = Operands((B, h, w, c), dev, split)
-        self.res_layers, self.res_out = [], []
-        prev = self.e[nd]
-        for i in range(self.repeat):
-            out = Operands((B, h, w, c), dev, split, f32=True)
-            l1 = self._make_layer(net.resnets[i].main[0], net.resnets[i].main[1], prev.pair, h=h, w=w, halo=(hm == 'all'))
-            l2 = self._make_layer(net.resnets[i].main[3], net.resnets[i].main[4], self.hb.pair, h=h, w=w, halo=(hm == 'all'))
-            self.res_layers.append((l1, l2))
-            self.res_out.append(out)
-            prev = out
-        # decoders + skippers
-        self.dec_layers, self.d_up, self.d_out = [], [], []
-        for i in range(nd):
-            up = Operands((B, h * 2, w * 2, c // 2), dev, split)
-            ld = self._make_layer(net.decoders[i][0], net.decoders[i][1], prev.pair, stride=2, transposed=True, h=h, w=w)
-            c, h, w = c // 2, h * 2, w * 2
-            last = (i == nd - 1)
-            tc_heads = (hm != '0') or (_tc_heads() and c == 64)
-            out = Operands((B, h, w, c), dev, split, f32=(last and not tc_heads), half=(not last or tc_heads))
-            ls = self._make_layer(net.skippers[i][0], net.skippers[i][1], self.e[nd - 1 - i].pair, x1=up.pair, h=h, w=w,
-                                  halo=(hm != '0'))
-            self.dec_layers.append((ld, ls))
-            self.d_up.append(up)
-            self.d_out.append(out)
-            prev = out
-        w_img, w_att = net.img_reg[0].weight.detach(), net.attetion_reg[0].weight.detach()
-        self.head_layer = None
-        self.folded_kw = 0
-        if hm == '0' and _tc_heads() and c == 64:
-            # img_reg (64->3) + attetion_reg (64->1): a 7 x 1 filter with N = 7 columns x 4 channels (-> 32) on the tensor
-            # cores; the composite kernel adds the seven column partials of every pixel (lwb_heads_composite, folded_kw)
-            self.head_layer = self._make_layer(None, None, prev.pair, h=H, w=W, weight=fold_head_weights(w_img, w_att),
-                                               pad=3, pad_w=0, n_tile=32)
-            self._stats_slots[-1] = 0
-            self.head_raw = self.head_layer.raw
-            self.folded_kw = 7
-        elif hm != '0':
-            # img_reg (64->3) + attetion_reg (64->1) as one 7x7 conv padded to 16 output channels on the
-            # tensor cores (halo variant, N tile 16); channels 0..3 are consumed by the composite kernel
-            w16 = torch.cat([w_img, w_att, torch.zeros(12, *w_img.shape[1:], device=w_img.device, dtype=w_img.dtype)], dim=0)
-            self.head_layer = self._make_layer(None, None, prev.pair, h=H, w=W, halo=True, weight=w16, pad=3, n_tile=16)
-            self._stats_slots[-1] = 0          # no InstanceNorm after the heads: no statistics
-            self.head_raw = self.head_layer.raw
-        else:
-            self.w4 = K.pack_head_weights(w_img, w_att)
-            self.head_raw = torch.empty((B, H, W, 4), dtype=torch.float32, device=dev)
-        self._finalize()
-        self._label_heads()
 
     # ---- pieces -------------------------------------------------------------------------
     def load_input(self, x):
@@ -387,7 +308,7 @@ class _UnetStream(_StreamBase):
             raise LwbError("unexpected input %s (stream built for %s)" % (tuple(x.shape), (self.B, self.cin, self.H, self.W)))
         K.nchw_to_nhwc_split(x.contiguous(), c_pad=8, pad_hw=(3, 3, 3, 5), hi=self.x_pad.hi, lo=self.x_pad.lo)
 
-    def encode(self, warp_srcs=None, T=None, ac=False, upto=None):
+    def encode(self, warp_srcs=None, T=None, ac=False):
         """encoders 0..n_down; warp_srcs[i] (NHWC fp32, i >= 1) is LWB-added after encoder i."""
         self.begin_pass()
         self._conv_norm(self.enc_layers[0], self.e[0], True)
@@ -419,104 +340,18 @@ class _UnetStream(_StreamBase):
             x = self.res_out[i]
 
     def decode(self):
-        for i, (ld, ls) in enumerate(self.dec_layers):
-            self._conv_norm(ld, self.d_up[i], True)
-            self._conv_norm(ls, self.d_out[i], True)
+        for (ld, ls), up, out in zip(self.dec_layers, self.d_up, self.d_out):
+            self._conv_norm(ld, up, True)
+            if ls is not None:
+                self._conv_norm(ls, out, True)
 
     def heads(self, bg=None, want_color=True, want_mask=True, **out):
-        if self.head_layer is not None:
-            self.head_layer.plan.run()
+        if self.head is not None:
+            self.head.plan.run()
         else:
             K.conv7x7_heads_nhwc(self.d_out[-1].f32, self.w4, out=self.head_raw)
         return K.heads_composite(self.head_raw, bg, want_color=want_color, want_mask=want_mask, folded_kw=self.folded_kw,
-                                 range_flag=self.range_flag if self.split == 2 else None, **out)
-
-    def encoder_outs_nchw(self):
-        outs = []
-        for a in self.e:
-            t = K.nhwc_to_nchw(a.f32)
-            t._lwb_nhwc = a.f32.clone()
-            outs.append(t)
-        return outs
-
-    def resnet_outs_nchw(self):
-        outs = []
-        for a in self.res_out:
-            t = K.nhwc_to_nchw(a.f32)
-            t._lwb_nhwc = a.f32.clone()
-            outs.append(t)
-        return outs
-
-
-class _ResnetStream(_StreamBase):
-    """ResNetGenerator (networks/generator.py:23-65, the BG net) bound to fixed shapes."""
-
-    def __init__(self, net, B, H, W, dev, split):
-        super(_ResnetStream, self).__init__(B, H, W, dev, split)
-        layers = list(net.model)
-        nd, rep = net._n_down, net._repeat_num
-        self.pitch = W + 8
-        self.x_pad = Operands((B, H + 6, self.pitch, 8), dev, split)
-        self.cin = layers[0].weight.shape[1]
-        if self.cin > 8:
-            raise LwbError("stem supports at most 8 input channels")
-        self.seq = []
-        i = 0
-        c, h, w = layers[0].weight.shape[0], H, W
-        out = Operands((B, h, w, c), dev, split)
-        self.seq.append(("cn", self._make_layer(layers[0], layers[1], self.x_pad.pair, rowk=True, row_pitch=self.pitch, h=H, w=W), out, True, None))
-        prev = out
-        i += 3
-        for k in range(nd):
-            out = Operands((B, h // 2, w // 2, c * 2), dev, split, f32=(k == nd - 1))
-            self.seq.append(("cn", self._make_layer(layers[i], layers[i + 1], prev.pair, stride=2, h=h, w=w), out, True, None))
-            c, h, w = c * 2, h // 2, w // 2
-            prev = out
-            i += 3
-        hb = Operands((B, h, w, c), dev, split)
-        for k in range(rep):
-            blk = layers[i]
-            out = Operands((B, h, w, c), dev, split, f32=True)
-            self.seq.append(("cn", self._make_layer(blk.main[0], blk.main[1], prev.pair, h=h, w=w), hb, True, None))
-            self.seq.append(("cn", self._make_layer(blk.main[3], blk.main[4], hb.pair, h=h, w=w), out, False, prev))
-            prev = out
-            i += 1
-        for k in range(nd):
-            last = (k == nd - 1)
-            tc_heads = _tc_heads() and c // 2 == 64
-            out = Operands((B, h * 2, w * 2, c // 2), dev, split, f32=(last and not tc_heads), half=(not last or tc_heads))
-            self.seq.append(("cn", self._make_layer(layers[i], layers[i + 1], prev.pair, stride=2, transposed=True, h=h, w=w), out, True, None))
-            c, h, w = c // 2, h * 2, w * 2
-            prev = out
-            i += 3
-        self.final = prev
-        w_img = layers[i].weight.detach()
-        self.head_layer = None
-        if _tc_heads() and c == 64:
-            self.head_layer = self._make_layer(None, None, prev.pair, h=H, w=W, pad=3, pad_w=0, n_tile=32,
-                                               weight=fold_head_weights(w_img, torch.zeros_like(w_img[:1])))
-            self._stats_slots[-1] = 0
-            self.head_raw = self.head_layer.raw
-        else:
-            self.w4 = K.pack_head_weights(w_img, torch.zeros_like(w_img[:1]))
-            self.head_raw = torch.empty((B, H, W, 4), dtype=torch.float32, device=dev)
-        self._finalize()
-        self._label_heads()
-
-    def run(self, x):
-        if tuple(x.shape) != (self.B, self.cin, self.H, self.W):
-            raise LwbError("unexpected input shape %s" % (tuple(x.shape),))
-        K.nchw_to_nhwc_split(x.float().contiguous(), c_pad=8, pad_hw=(3, 3, 3, 5), hi=self.x_pad.hi, lo=self.x_pad.lo)
-        self.begin_pass()
-        for _, L, out, relu, res in self.seq:
-            self._conv_norm(L, out, relu, residual=(res.f32 if res is not None else None))
-        if self.head_layer is not None:
-            self.head_layer.plan.run()
-        else:
-            K.conv7x7_heads_nhwc(self.final.f32, self.w4, out=self.head_raw)
-        color, _, _ = K.heads_composite(self.head_raw, None, want_color=True, want_mask=False,
-                                        folded_kw=7 if self.head_layer is not None else 0)
-        return color
+                                 range_flag=self.head_flag, **out)
 
 
 def profile_streams(warm_fn, run_fn):
@@ -546,6 +381,16 @@ def _nhwc_of(t):
     if cached is not None:
         return cached
     return t.permute(0, 2, 3, 1).contiguous()
+
+
+def _nchw_outs(acts):
+    """NCHW copies of the fp32 activations, each carrying its NHWC twin for _nhwc_of."""
+    outs = []
+    for a in acts:
+        t = K.nhwc_to_nchw(a.f32)
+        t._lwb_nhwc = a.f32.clone()
+        outs.append(t)
+    return outs
 
 
 class ResNetGenerator(NetworkBase):
@@ -587,8 +432,12 @@ class ResNetGenerator(NetworkBase):
             x = torch.cat([x, c], dim=1)
         B, _, H, W = x.shape
         split = split_mode(self)
-        st = _stream_for(self, _ResnetStream, ('bg', B, H, W, split), B, H, W, x.device, split)
-        return st.run(x)
+        st = _stream_for(self, _Stream, ('bg', B, H, W, split), B, H, W, x.device, split)
+        st.load_input(x.float())
+        st.encode()
+        st.resnets()
+        st.decode()
+        return st.heads(want_mask=False)[0]
 
 
 class ResUnetGenerator(NetworkBase):
@@ -643,7 +492,7 @@ class ResUnetGenerator(NetworkBase):
     def _stream(self, x, keep_f32, tag):
         B, _, H, W = x.shape
         split = split_mode(self)
-        return _stream_for(self, _UnetStream, (tag, B, H, W, split, keep_f32), B, H, W, x.device, split, keep_f32=keep_f32)
+        return _stream_for(self, _Stream, (tag, B, H, W, split, keep_f32), B, H, W, x.device, split, keep_f32=keep_f32)
 
     @torch.no_grad()
     def inference(self, x):
@@ -652,7 +501,7 @@ class ResUnetGenerator(NetworkBase):
         st.load_input(x.float())
         st.encode()
         st.resnets()
-        return st.encoder_outs_nchw(), st.resnet_outs_nchw()
+        return _nchw_outs(st.e), _nchw_outs(st.res_out)
 
     @torch.no_grad()
     def forward(self, x):
@@ -698,7 +547,7 @@ class ImpersonatorGenerator(NetworkBase):
 
     @torch.no_grad()
     def infer_front(self, src_inputs, tsf_inputs, T):
-        ac = _align_corners()
+        ac = K.default_align_corners()
         _new_pass()
         T = T.float().contiguous()
         src = self.src_model._stream(src_inputs, True, 'front')
@@ -719,7 +568,7 @@ class ImpersonatorGenerator(NetworkBase):
     def swap(self, tsf_inputs, src_encoder_outs12, src_encoder_outs21, src_resnet_outs12, src_resnet_outs21, T12, T21, bg=None):
         """networks/generator.py:245-275.  With ``bg`` (extension) also returns the composite m*bg + (1-m)*color of
         models/swapper.py:268-269 from the head kernel."""
-        ac = _align_corners()
+        ac = K.default_align_corners()
         _new_pass()
         T12, T21 = T12.float().contiguous(), T21.float().contiguous()
         tsf = self.tsf_model._stream(tsf_inputs, True, 'swap')
@@ -740,7 +589,7 @@ class ImpersonatorGenerator(NetworkBase):
         models/imitator.py:331 as a third value (fused into the head kernel); ``pred_hwc`` / ``pred_u8``
         (caller-allocated [B,H,W,3] float32 / uint8-BGR) receive the same frames in the layouts of the output
         path (models/imitator.py:178-180, utils/cv_utils.py:23-36) from that launch."""
-        ac = _align_corners()
+        ac = K.default_align_corners()
         _new_pass()
         if (pred_hwc is not None or pred_u8 is not None) and bg is None:
             raise LwbError("pred_hwc / pred_u8 need bg (they hold the composite)")
@@ -805,8 +654,8 @@ class ImpersonatorGenerator(NetworkBase):
 
     @torch.no_grad()
     def stn(self, x, T):
-        return K.warp_nchw(x.float().contiguous(), T.float().contiguous(), align_corners=_align_corners())
+        return K.warp_nchw(x.float().contiguous(), T.float().contiguous(), align_corners=K.default_align_corners())
 
     @torch.no_grad()
     def transform(self, x, T):
-        return K.warp_nchw(x.float().contiguous(), T.float().contiguous(), align_corners=_align_corners())
+        return K.warp_nchw(x.float().contiguous(), T.float().contiguous(), align_corners=K.default_align_corners())

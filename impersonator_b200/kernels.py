@@ -222,8 +222,6 @@ def pack_conv_weight(w, transposed=False, cout_pad=None, cin_pad=None, split=Tru
     hi+lo, 2 fp16 hi + fp8 pair blocks (lwb_pack_conv_weight_f8).  ``absmax`` = max|w| when the caller already knows it
     (one host sync per network instead of one per layer); computed here otherwise."""
     _chk_cuda(w)
-    if int(split) == 2:
-        return _pack_conv_weight_f8(w, transposed, cout_pad, cin_pad, absmax)
     w = w.float().contiguous()
     if transposed:
         cin, cout, kh, kw = w.shape
@@ -233,25 +231,10 @@ def pack_conv_weight(w, transposed=False, cout_pad=None, cin_pad=None, split=Tru
     cin_pad = cin_pad or cin
     w_exp = weight_exponent(w.abs().max() if absmax is None else absmax)
     hi = torch.empty((kh * kw, cout_pad, cin_pad), dtype=torch.float16, device=w.device)
-    lo = torch.empty_like(hi) if split else None
-    check(lib().lwb_pack_conv_weight(ptr(w), cout, cin, kh, kw, 1 if transposed else 0, cout_pad, cin_pad, w_exp,
-                                     ptr(hi), ptr(lo), stream()), "lwb_pack_conv_weight")
-    return PackedWeight(hi, lo, w_exp)
-
-
-def _pack_conv_weight_f8(w, transposed, cout_pad, cin_pad, absmax=None):
-    w = w.float().contiguous()
-    if transposed:
-        cin, cout, kh, kw = w.shape
-    else:
-        cout, cin, kh, kw = w.shape
-    cout_pad = cout_pad or cout
-    cin_pad = cin_pad or cin
-    w_exp = weight_exponent(w.abs().max() if absmax is None else absmax)
-    hi = torch.empty((kh * kw, cout_pad, cin_pad), dtype=torch.float16, device=w.device)
-    lo = torch.empty_like(hi)                                   # same bytes, fp8 pair blocks inside
-    check(lib().lwb_pack_conv_weight_f8(ptr(w), cout, cin, kh, kw, 1 if transposed else 0, cout_pad, cin_pad, w_exp,
-                                        ptr(hi), ptr(lo), stream()), "lwb_pack_conv_weight_f8")
+    lo = torch.empty_like(hi) if split else None                # split 2: same bytes, fp8 pair blocks inside
+    entry = "lwb_pack_conv_weight_f8" if int(split) == 2 else "lwb_pack_conv_weight"
+    check(getattr(lib(), entry)(ptr(w), cout, cin, kh, kw, 1 if transposed else 0, cout_pad, cin_pad, w_exp,
+                                ptr(hi), ptr(lo), stream()), entry)
     return PackedWeight(hi, lo, w_exp)
 
 

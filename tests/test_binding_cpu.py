@@ -48,15 +48,20 @@ def test_inception_stream_matches_oracle(monkeypatch):
 def test_every_stream_packs_with_a_known_absmax(monkeypatch):
     """Each stream reads max|w| of all its layers in one host sync before packing: no pack call computes it itself."""
     from impersonator_b200.detectors import MaskRCNN, _DetStream
+    from impersonator_b200.generator import ImpersonatorGenerator
     from impersonator_b200.hmr import HumanModelRecovery, _HmrStream
     from impersonator_b200.inpaintor import InpaintSANet, _InpaintStream
     _cpu_metrics(monkeypatch)
     calls = []
 
-    def pack(w, *args, **kw):
-        calls.append(kw.get("absmax"))
-        return kernel_emulator.pack_conv_weight(w, *args, **kw)
-    monkeypatch.setattr(K, "pack_conv_weight", pack)
+    def recorded(pack):
+        def f(w, *args, **kw):
+            calls.append(kw.get("absmax"))
+            return pack(w, *args, **kw)
+        return f
+    monkeypatch.setattr(K, "pack_conv_weight", recorded(kernel_emulator.pack_conv_weight))
+    monkeypatch.setattr(K, "pack_conv_weight_rowk", recorded(kernel_emulator.pack_conv_weight_rowk))
+    gen = ImpersonatorGenerator(bg_dim=4, src_dim=6, tsf_dim=6, repeat_num=6).eval()
     gold = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "inception.npz"))
     convs, lins = MC.synthetic_alexnet(), MC.synthetic_lins()
     builds = {
@@ -66,6 +71,8 @@ def test_every_stream_packs_with_a_known_absmax(monkeypatch):
         "lpips": lambda: M._AlexStream(M.LPIPS(weights=MC.alexnet_state_dict(convs), lin_weights=MC.lin_state_dict(lins)),
                                        1, 64, 64, CPU),
         "inception": lambda: M.InceptionFeatures(weights=IC.golden_state_dict(gold)).stream(1, 64, 64),
+        "unet": lambda: gen.tsf_model(torch.zeros(1, 6, 64, 64)),
+        "bg": lambda: gen.bg_model(torch.zeros(1, 4, 64, 64)),
     }
     counts = {}
     for name, build in builds.items():
@@ -73,4 +80,6 @@ def test_every_stream_packs_with_a_known_absmax(monkeypatch):
         build()
         assert calls and all(isinstance(a, float) for a in calls), (name, calls)
         counts[name] = len(calls)
-    assert counts == dict(hmr=52, inpaintor=36, detector=79, lpips=4, inception=65), counts
+    # the generator streams with the default (folded tensor-core) heads: stem, 3 encoders, 6 x 2 residual convs,
+    # 3 decoders, 3 skippers (not in the BG net), heads
+    assert counts == dict(hmr=52, inpaintor=36, detector=79, lpips=4, inception=65, unet=23, bg=20), counts

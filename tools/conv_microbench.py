@@ -32,7 +32,7 @@ def load(tree):
     global K, merge_transposed_weight
     sys.path.insert(0, os.path.abspath(tree))
     from impersonator_b200 import kernels
-    from impersonator_b200.generator import merge_transposed_weight as mtw
+    from impersonator_b200.binding import merge_transposed_weight as mtw
     K, merge_transposed_weight = kernels, mtw
 
 TILE_H, TILE_W, KCHUNK, MAX_GROUP = 16, 8, 64, 8
