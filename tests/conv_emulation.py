@@ -102,6 +102,26 @@ def check_stats(st, got):
     assert e1 <= STATS_BAR and e2 <= STATS_BAR
 
 
+BAND = 1 << 18                  # bytes of sentinel before and after each view (a multiple of 256: the views stay aligned)
+SENTINEL = 0xA5
+
+
+def guarded(cuda, shape, dtype, fill):
+    """A contiguous ``shape`` view of ``dtype`` inside a byte buffer with BAND sentinel bytes on each side."""
+    nbytes = torch.Size(shape).numel() * torch.empty((), dtype=dtype).element_size()
+    buf = torch.full((BAND + nbytes + BAND,), SENTINEL, dtype=torch.uint8, device=cuda)
+    view = buf[BAND:BAND + nbytes].view(dtype).view(shape)
+    view.fill_(fill)
+    return buf, view
+
+
+def assert_bands_intact(name, buf):
+    for side, band in (("before", buf[:BAND]), ("after", buf[-BAND:])):
+        bad = (band != SENTINEL).nonzero()
+        assert bad.numel() == 0, "%s: %d sentinel bytes %s the view were overwritten (first at %d)" % (
+            name, bad.numel(), side, int(bad[0]) if bad.numel() else -1)
+
+
 def check_conv(name, split, got, x, w, conv, w_exp, stats=None, emu_bar=EMU_BAR):
     """The checks of one conv-engine result ``got`` (NCHW fp32, CPU) of ``conv(x, w)`` in operand mode ``split``:
     (a) against the mode's float64 emulation, (b) against fp32, (c) the statistics against ``got`` itself."""

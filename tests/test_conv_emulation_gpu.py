@@ -15,7 +15,7 @@ import torch
 import torch.nn.functional as F
 
 from impersonator_b200 import kernels as K
-from conv_emulation import check_conv, report
+from conv_emulation import assert_bands_intact, check_conv, guarded, report
 from test_conv_gpu import rnd, run_conv, run_merged_transposed, run_stem
 
 pytestmark = pytest.mark.gpu
@@ -43,26 +43,6 @@ def test_conv_one_past_tile_boundary(cuda, case, split):
 
 
 # ----------------------------------------------------------------------------------------------------------- canaries
-BAND = 1 << 18                  # bytes of sentinel before and after each view (a multiple of 256: the views stay aligned)
-SENTINEL = 0xA5
-
-
-def guarded(cuda, shape, dtype, fill):
-    """A contiguous ``shape`` view of ``dtype`` inside a byte buffer with BAND sentinel bytes on each side."""
-    nbytes = torch.Size(shape).numel() * torch.empty((), dtype=dtype).element_size()
-    buf = torch.full((BAND + nbytes + BAND,), SENTINEL, dtype=torch.uint8, device=cuda)
-    view = buf[BAND:BAND + nbytes].view(dtype).view(shape)
-    view.fill_(fill)
-    return buf, view
-
-
-def assert_bands_intact(name, buf):
-    for side, band in (("before", buf[:BAND]), ("after", buf[-BAND:])):
-        bad = (band != SENTINEL).nonzero()
-        assert bad.numel() == 0, "%s: %d sentinel bytes %s the view were overwritten (first at %d)" % (
-            name, bad.numel(), side, int(bad[0]) if bad.numel() else -1)
-
-
 CANARY_CASES = ["partial_plain", "swapped", "transposed_phases", "transposed_merged"]
 
 

@@ -6,7 +6,7 @@ import torch
 
 from impersonator_b200 import kernels as K
 import glue_cases as G
-from test_conv_emulation_gpu import assert_bands_intact, guarded
+from conv_emulation import assert_bands_intact, guarded
 
 pytestmark = pytest.mark.gpu
 

@@ -6,7 +6,7 @@ import torch
 
 import glue_cases as G
 from impersonator_b200._lib import check, lib, ptr, stream
-from test_conv_emulation_gpu import assert_bands_intact, guarded
+from conv_emulation import assert_bands_intact, guarded
 
 pytestmark = pytest.mark.gpu
 
