@@ -12,6 +12,11 @@ from ._lib import LwbError
 
 DEFAULT_PRECISION = "fp16f8"
 
+# Bits of the operand-range flag (LWB_RANGE_* of include/lwb_b200.h)
+RANGE_F8 = 1            # an emitted operand has |x| >= 1024: its e4m3 correction terms clip
+RANGE_FP16 = 2          # |x| >= 60000 or not finite: the fp16 hi itself overflows
+RANGE_HEADS = 4         # a head pre-activation reached +-8
+
 
 def precision_mode():
     return os.environ.get("LWB_PRECISION", DEFAULT_PRECISION)
@@ -27,6 +32,12 @@ def split_mode(mod=None):
     if mode not in codes:
         raise LwbError("LWB_PRECISION must be fp16x3, fp16f8 or fp16")
     return codes[mode]
+
+
+def lo_format(split):
+    """The lo operand format the epilogues emit for conv plans of operand mode ``split``: 1 (fp8 pair blocks) for
+    fp16f8, else 0 (fp16)."""
+    return 1 if split == 2 else 0
 
 
 class Operands(object):

@@ -60,10 +60,4 @@ __device__ __forceinline__ void stg_f32x8(float* p, const float* v) {
     reinterpret_cast<float4*>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
 }
 
-// x ~= hi + lo with hi = fp16(x), lo = fp16(x - hi): the 2-term operand split of the conv engine.
-__device__ __forceinline__ void split_half(float x, __half& hi, __half& lo) {
-    hi = __float2half_rn(x);
-    lo = __float2half_rn(x - __half2float(hi));
-}
-
 }  // namespace lwb

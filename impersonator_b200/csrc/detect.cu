@@ -12,6 +12,7 @@
 #include <cub/block/block_scan.cuh>
 
 #include "common.cuh"
+#include "operands.cuh"
 
 namespace {
 
@@ -30,16 +31,7 @@ __device__ __forceinline__ unsigned int order_key(float f)
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
-__device__ __forceinline__ void store_operand(float v, size_t i, float* y_f32, __half* y_hi, __half* y_lo)
-{
-    if (y_f32) y_f32[i] = v;
-    if (y_hi) {
-        __half h, l;
-        lwb::split_half(v, h, l);
-        y_hi[i] = h;
-        if (y_lo) y_lo[i] = l;
-    }
-}
+using lwb::store_operand;
 
 // ---- GeneralizedRCNNTransform: (x + 1) / 2, normalise, bilinear resize (align_corners=False), zero pad ----------------
 __global__ void k_det_transform(const float* __restrict__ img, int h, int w, int ho, int wo, int hp, int wp, float sy, float sx,

@@ -3,9 +3,8 @@
 //
 // networks/generator.py:8-20 (ResidualBlock), :80-95 (Conv+IN+ReLU), :283-295 (tsf + warp),
 // :183-184 (tanh / sigmoid heads), models/imitator.py:330-331 (composite).
-#include <cuda_fp8.h>
-
 #include "common.cuh"
+#include "operands.cuh"
 #include "sample.cuh"
 
 namespace {
@@ -13,11 +12,14 @@ namespace {
 using lwb::split_half;
 
 // ---------------------------------------------------------------------------------------------
-// weights: OIHW (Conv2d) / IOHW (ConvTranspose2d) fp32 -> [tap][cout_pad][cin_pad] fp16 hi/lo of w * 2^E
+// weights: OIHW (Conv2d) / IOHW (ConvTranspose2d) fp32 -> [tap][cout_pad][cin_pad] hi = fp16 of w * 2^E and
+//   LO_FORMAT 0: lo (nullable) = the fp16 residual of w * 2^E;
+//   LO_FORMAT 1: hi = fp16(w_hi) * 2^E, lo = the pair blocks [64 x e4m3(w_lo * 2^(E+4))][64 x e4m3(w * 2^(E-10))]
 // (wscale = 2^E, the layer's exponent: max|w| * 2^E in [2^14, 2^15) keeps hi and lo out of the fp16 subnormals)
 // ---------------------------------------------------------------------------------------------
+template <int LO_FORMAT>
 __global__ void k_pack_weight(const float* __restrict__ w, int cout, int cin, int kh, int kw, int transposed,
-                              int cout_pad, int cin_pad, float wscale, __half* __restrict__ hi, __half* __restrict__ lo)
+                              int cout_pad, int cin_pad, float wscale, __half* __restrict__ hi, void* __restrict__ lo)
 {
     const long total = (long)kh * kw * cout_pad * cin_pad;
     for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -30,51 +32,18 @@ __global__ void k_pack_weight(const float* __restrict__ w, int cout, int cin, in
             v = transposed ? w[(((size_t)ci * cout + co) * kh + ky) * kw + kx]
                            : w[(((size_t)co * cin + ci) * kh + ky) * kw + kx];
         }
-        __half h, l;
-        split_half(v * wscale, h, l);
-        hi[i] = h;
-        if (lo) lo[i] = l;
-    }
-}
-
-// fp8 scales of the "fp16 + fp8" operand split (conv_tc.cu, f8 mode).  With hi = fp16(v), lo = v - hi:
-//     x * w ~= x_hi * w_hi + x * w_lo + x_lo * w            (the two small products only need ~4 bits)
-// and everything is accumulated 2^E too large so that no fp8 operand underflows; E is chosen PER LAYER so that
-// max|w| * 2^E lies in [2^14, 2^15) (lwb_conv_desc.w_exp; any weight magnitude packs without overflow):
-//     A_hi = x_hi                           B_hi  = fp16(w_hi * 2^E)          (exact: a power of two)
-//     A_lo8[0:64]   = e4m3(x * 2^-4)        B_lo8[0:64]   = e4m3(w_lo * 2^(E+4))     |.| <= 2^8
-//     A_lo8[64:128] = e4m3(x_lo * 2^10)     B_lo8[64:128] = e4m3(w * 2^(E-10))       |.| <  2^5
-// per 64-channel block (one 128 B K row); the epilogue multiplies by 2^-E.  Activation range: e4m3 saturates at 448,
-// i.e. x_lo (<= half an fp16 ulp of x) clips for |x| >= 1024 and x itself for |x| >= 7168 -- the split then degrades
-// gracefully towards single-pass fp16 for those elements; k_norm_act reports it through its range flag
-// (bit 0: |y| >= 1024, bit 1: |y| >= 60000 or non-finite = the fp16 hi operand itself overflows).
-constexpr float kF8XScale = 1.f / 16.f, kF8XLoScale = 1024.f;
-constexpr float kF8WLoRel = 16.f, kF8WRel = 1.f / 1024.f;       // relative to the layer's 2^E
-
-__device__ __forceinline__ uint8_t to_e4m3(float v) { return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3); }
-
-// weights, f8 mode: hi [tap][cout_pad][cin_pad] fp16 = w_hi * 2^E;  lo8: the same 2 bytes per element, per 64-channel
-// block [64 x e4m3(w_lo * 2^(E+4))][64 x e4m3(w * 2^(E-10))]
-__global__ void k_pack_weight_f8(const float* __restrict__ w, int cout, int cin, int kh, int kw, int transposed,
-                                 int cout_pad, int cin_pad, float wscale, __half* __restrict__ hi, uint8_t* __restrict__ lo8)
-{
-    const long total = (long)kh * kw * cout_pad * cin_pad;
-    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        const int ci = (int)(i % cin_pad);
-        const int co = (int)((i / cin_pad) % cout_pad);
-        const int tap = (int)(i / ((long)cin_pad * cout_pad));
-        float v = 0.f;
-        if (ci < cin && co < cout) {
-            const int ky = tap / kw, kx = tap % kw;
-            v = transposed ? w[(((size_t)ci * cout + co) * kh + ky) * kw + kx]
-                           : w[(((size_t)co * cin + ci) * kh + ky) * kw + kx];
+        if (LO_FORMAT == 1) {
+            const __half h = __float2half_rn(v);
+            hi[i] = __float2half_rn(__half2float(h) * wscale);         // exact: |w| * 2^E < 2^15 (host picks E)
+            uint8_t* blk = lwb::pair_block(lo, i, ci);
+            blk[0] = lwb::to_e4m3((v - __half2float(h)) * (wscale * lwb::kF8WLoRel));
+            blk[64] = lwb::to_e4m3(v * (wscale * lwb::kF8WRel));
+        } else {
+            __half h, l;
+            split_half(v * wscale, h, l);
+            hi[i] = h;
+            if (lo) static_cast<__half*>(lo)[i] = l;
         }
-        const __half h = __float2half_rn(v);
-        const float lo = v - __half2float(h);
-        hi[i] = __float2half_rn(__half2float(h) * wscale);             // exact: |w| * 2^E < 2^15 (host picks E)
-        uint8_t* blk = lo8 + (i - ci) * 2 + (size_t)(ci / 64) * 128;
-        blk[ci % 64] = to_e4m3(lo * (wscale * kF8WLoRel));
-        blk[64 + ci % 64] = to_e4m3(v * (wscale * kF8WRel));
     }
 }
 
@@ -212,8 +181,8 @@ struct NormActParams {
     const float* residual;
     const float* warp_src; int src_batch; const float* T; int th, tw, align_corners;
     float* y_f32; __half* y_hi; __half* y_lo;
-    int lo_format;                                       // 0: y_lo = fp16 residual; 1: fp8 pair blocks (see kF8* above)
-    int* range_flag;                                     // |= 1 / 2 when an emitted operand leaves the f8 / fp16 range
+    int lo_format;                                       // 0: y_lo = fp16 residual; 1: fp8 pair blocks (operands.cuh)
+    int* range_flag;                                     // |= lwb::range_bits of the emitted operands
     // EXT only (BatchNorm-style nets, networks/hmr.py): the operands are relu?(y * post_scale[c] + post_shift[c]) while
     // y_f32 keeps y; the residual is read at (res_step*y, res_step*x) of a [n, h*res_step, w*res_step, c] tensor
     const float* post_scale; const float* post_shift; int post_relu; int res_step;
@@ -349,34 +318,9 @@ __global__ void __launch_bounds__(256, 4) k_norm_act(NormActParams P)
                     if (P.post_relu) v[r][k] = fmaxf(v[r][k], 0.f);
                 }
             }
-            __align__(16) __half hh[8];
-            __align__(16) __half ll[8];
-#pragma unroll
-            for (int k = 0; k < 8; k++) split_half(v[r][k], hh[k], ll[k]);
-            const uint4 hv = *reinterpret_cast<const uint4*>(hh);
-            if (P.range_flag) {
-                // max |hi| of the eight fp16 values as integers (monotone in |x|; inf / NaN sort above everything)
-                unsigned m = __vmaxu2(__vmaxu2(hv.x & 0x7fff7fffu, hv.y & 0x7fff7fffu), __vmaxu2(hv.z & 0x7fff7fffu, hv.w & 0x7fff7fffu));
-                m = max(m & 0xffffu, m >> 16);
-                if (m >= 0x6400u) atomicOr(P.range_flag, m >= 0x7b53u ? 3 : 1);       // fp16 1024.0 / 60000
-            }
-            *reinterpret_cast<uint4*>(P.y_hi + off[r]) = hv;
-            if (P.y_lo && P.lo_format == 0) {
-                *reinterpret_cast<uint4*>(P.y_lo + off[r]) = *reinterpret_cast<const uint4*>(ll);
-            } else if (P.y_lo) {
-                __align__(8) uint8_t x8[8];
-                __align__(8) uint8_t l8[8];
-#pragma unroll
-                for (int k = 0; k < 8; k++) {
-                    x8[k] = to_e4m3(v[r][k] * kF8XScale);
-                    l8[k] = to_e4m3((v[r][k] - __half2float(hh[k])) * kF8XLoScale);
-                }
-                // channel c of this pixel lives in 64-channel block c / 64: bytes [c % 64] and [64 + c % 64]
-                const int ch = g * 8;
-                uint8_t* blk = reinterpret_cast<uint8_t*>(P.y_lo) + (off[r] - ch) * 2 + (size_t)(ch / 64) * 128 + (ch % 64);
-                *reinterpret_cast<uint2*>(blk) = *reinterpret_cast<const uint2*>(x8);
-                *reinterpret_cast<uint2*>(blk + 64) = *reinterpret_cast<const uint2*>(l8);
-            }
+            const lwb::Operand8 e = lwb::encode8(v[r], 0);
+            if (P.range_flag) { if (const int bits = lwb::range_bits(e.hi)) atomicOr(P.range_flag, bits); }
+            lwb::store8(e, v[r], P.y_hi, P.y_lo, P.lo_format, off[r], g * 8);
         }
     }
 }
@@ -417,10 +361,11 @@ __global__ void __launch_bounds__(256) k_heads(const float* __restrict__ raw, in
     }
     if (range_flag) {
         // Output-head pre-activations of +-8 and more: the ~1e-4 end-to-end RELATIVE precision of the fp16f8 operand split is
-        // then no longer enough for 1e-3 on the (unsaturated) pixels -- report it (bit 2), the caller switches to fp16x3.
+        // then no longer enough for 1e-3 on the (unsaturated) pixels -- report it, the caller switches to fp16x3.
         // (fmaxf would drop a NaN component, so each one is compared on its own)
         const bool big = !(fabsf(r.x) < 8.f && fabsf(r.y) < 8.f && fabsf(r.z) < 8.f && fabsf(r.w) < 8.f);
-        if (__any_sync(__activemask(), big) && big && !(*reinterpret_cast<volatile int*>(range_flag) & 4)) atomicOr(range_flag, 4);
+        if (__any_sync(__activemask(), big) && big && !(*reinterpret_cast<volatile int*>(range_flag) & LWB_RANGE_HEADS))
+            atomicOr(range_flag, LWB_RANGE_HEADS);
     }
     const float col[3] = {tanhf(r.x), tanhf(r.y), tanhf(r.z)};
     const float m = 1.f / (1.f + expf(-r.w));
@@ -494,8 +439,8 @@ extern "C" int lwb_pack_conv_weight(const float* w, int cout, int cin, int kh, i
     LWB_CHECK_ARG(cout > 0 && cin > 0 && kh > 0 && kw > 0 && cout_pad >= cout && cin_pad >= cin, "bad sizes");
     LWB_CHECK_ARG(w_exp >= -40 && w_exp <= 60, "w_exp out of range");
     const long total = (long)kh * kw * cout_pad * cin_pad;
-    k_pack_weight<<<(int)min((total + 255) / 256, 4096l), 256, 0, (cudaStream_t)stream>>>(
-        w, cout, cin, kh, kw, transposed, cout_pad, cin_pad, ldexpf(1.f, w_exp), (__half*)w_hi, (__half*)w_lo);
+    k_pack_weight<0><<<(int)min((total + 255) / 256, 4096l), 256, 0, (cudaStream_t)stream>>>(
+        w, cout, cin, kh, kw, transposed, cout_pad, cin_pad, ldexpf(1.f, w_exp), (__half*)w_hi, w_lo);
     LWB_LAUNCH_OK();
     return LWB_OK;
 }
@@ -507,7 +452,7 @@ extern "C" int lwb_pack_conv_weight_f8(const float* w, int cout, int cin, int kh
     LWB_CHECK_ARG(cout > 0 && cin > 0 && kh > 0 && kw > 0 && cout_pad >= cout && cin_pad >= cin && (cin_pad % 64) == 0, "bad sizes");
     LWB_CHECK_ARG(w_exp >= -40 && w_exp <= 60, "w_exp out of range");
     const long total = (long)kh * kw * cout_pad * cin_pad;
-    k_pack_weight_f8<<<(int)min((total + 255) / 256, 4096l), 256, 0, (cudaStream_t)stream>>>(
+    k_pack_weight<1><<<(int)min((total + 255) / 256, 4096l), 256, 0, (cudaStream_t)stream>>>(
         w, cout, cin, kh, kw, transposed, cout_pad, cin_pad, ldexpf(1.f, w_exp), (__half*)w_hi, w_lo8);
     LWB_LAUNCH_OK();
     return LWB_OK;

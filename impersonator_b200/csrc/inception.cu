@@ -3,6 +3,7 @@
 // conv engine (lwb_conv_plan_*) and the stem on lwb_conv2d_direct_relu_nhwc; the pools are lwb_maxpool_nhwc(_slice) and
 // lwb_global_avgpool_nhwc.  No reduction here depends on scheduling, so the features repeat bit for bit.
 #include "common.cuh"
+#include "operands.cuh"
 
 namespace {
 
@@ -69,14 +70,7 @@ __global__ void __launch_bounds__(THREADS) k_bn_act_segment(const float* __restr
         v = scale ? fmaf(r, __ldg(scale + ch), __ldg(shift + ch)) : r;
         if (relu) v = fmaxf(v, 0.f);
     }
-    const size_t o = (size_t)pix * ld_y + off_y + ch;
-    if (y_f32) y_f32[o] = v;
-    if (y_hi) {
-        __half hi, lo;
-        lwb::split_half(v, hi, lo);
-        y_hi[o] = hi;
-        if (y_lo) y_lo[o] = lo;
-    }
+    lwb::store_operand(v, (size_t)pix * ld_y + off_y + ch, y_f32, y_hi, y_lo);
 }
 
 }  // namespace

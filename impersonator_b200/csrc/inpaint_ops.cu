@@ -5,15 +5,10 @@
 //                 2x grid that GatedDeConv2dWithActivation convolves (:65-68), optionally clamped to [-1, 1] (:187,196)
 //   k_self_attention  SelfAttention (:86-107): softmax(Q K^T) V over all N = H*W positions, flash-style (online softmax,
 //                 K / V tiles in shared memory), fp32 on the CUDA cores: 2 N^2 (16 + 128) = 4.8 GFLOP per image
-#include <cuda_fp8.h>
-
 #include "common.cuh"
+#include "operands.cuh"
 
 namespace {
-
-using lwb::split_half;
-
-__device__ __forceinline__ uint8_t f8(float v) { return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3); }
 
 struct GatedParams {
     const float* raw; int n, h, w, c, c_stride;          // raw [n,h,w,c_stride]: a = [0,c), b = [c,2c)
@@ -56,22 +51,8 @@ __global__ void __launch_bounds__(256) k_gated_act(GatedParams P)
         }
         v[k] = out;
     }
-    __align__(16) __half hh[8];
-    __align__(16) __half ll[8];
-    __align__(8) uint8_t x8[8];
-    __align__(8) uint8_t l8[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-        split_half(v[k], hh[k], ll[k]);
-        x8[k] = f8(v[k] * (1.f / 16.f));
-        l8[k] = f8((v[k] - __half2float(hh[k])) * 1024.f);             // the f8 pair block scales of elementwise.cu
-    }
-    const uint4 hv = *reinterpret_cast<const uint4*>(hh);
-    if (P.range_flag && P.y_hi) {
-        unsigned m = __vmaxu2(__vmaxu2(hv.x & 0x7fff7fffu, hv.y & 0x7fff7fffu), __vmaxu2(hv.z & 0x7fff7fffu, hv.w & 0x7fff7fffu));
-        m = max(m & 0xffffu, m >> 16);
-        if (m >= 0x6400u) atomicOr(P.range_flag, m >= 0x7b53u ? 3 : 1);
-    }
+    const lwb::Operand8 e = lwb::encode8(v, P.lo_format);
+    if (P.range_flag && P.y_hi) { if (const int bits = lwb::range_bits(e.hi)) atomicOr(P.range_flag, bits); }
     const int ho = P.h * P.up, wo = P.w * P.up;
     for (int dy = 0; dy < P.up; dy++) for (int dx = 0; dx < P.up; dx++) {
         const size_t opix = ((size_t)b * ho + (size_t)y * P.up + dy) * wo + (size_t)x * P.up + dx;
@@ -79,18 +60,7 @@ __global__ void __launch_bounds__(256) k_gated_act(GatedParams P)
 #pragma unroll
             for (int k = 0; k < 8; k++) if (g * 8 + k < P.c) P.y_f32[opix * P.f32_stride + g * 8 + k] = v[k];
         }
-        if (P.y_hi) {
-            const size_t off = opix * P.c_pad + g * 8;
-            *reinterpret_cast<uint4*>(P.y_hi + off) = hv;
-            if (P.y_lo && P.lo_format == 0) {
-                *reinterpret_cast<uint4*>(P.y_lo + off) = *reinterpret_cast<const uint4*>(ll);
-            } else if (P.y_lo) {
-                const int ch = g * 8;
-                uint8_t* blk = reinterpret_cast<uint8_t*>(P.y_lo) + (off - ch) * 2 + (size_t)(ch / 64) * 128 + (ch % 64);
-                *reinterpret_cast<uint2*>(blk) = *reinterpret_cast<const uint2*>(x8);
-                *reinterpret_cast<uint2*>(blk + 64) = *reinterpret_cast<const uint2*>(l8);
-            }
-        }
+        if (P.y_hi) lwb::store8(e, nullptr, P.y_hi, P.y_lo, P.lo_format, opix * P.c_pad + g * 8, g * 8);
     }
 }
 

@@ -3,6 +3,7 @@
 // iterative theta regressor.  All three are far from any roofline-relevant size (per image: 0.8 M max-pool
 // outputs, a 49 x 2048 mean, 3 x 3.3 M multiply-adds); they exist so that no torch operator sits on the path.
 #include "common.cuh"
+#include "operands.cuh"
 
 namespace {
 
@@ -50,14 +51,7 @@ __global__ void __launch_bounds__(256) k_maxpool_nhwc(const float* __restrict__ 
     for (int dy = 0; dy < k; dy++)
         for (int dx = 0; dx < k; dx++)
             m = fmaxf(m, __ldg(p + ((size_t)dy * w + dx) * ld_x));
-    const size_t o = (size_t)pix * ld_y + off_y + ch;
-    if (y_f32) y_f32[o] = m;
-    if (y_hi) {
-        __half hi, lo;
-        lwb::split_half(m, hi, lo);
-        y_hi[o] = hi;
-        if (y_lo) y_lo[o] = lo;
-    }
+    lwb::store_operand(m, (size_t)pix * ld_y + off_y + ch, y_f32, y_hi, y_lo);
 }
 
 // out[b, ch] = mean over hw of relu?(x[b, p, ch] * scale[ch] + shift[ch])   (post_bn + ReLU + avg_pool2d(7), hmr.py:160-163)

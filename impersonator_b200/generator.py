@@ -31,7 +31,7 @@ import torch.nn as nn
 
 from . import kernels as K
 from ._lib import LwbError
-from .binding import Operands, PlanBinder, StreamOwner, precision_mode, split_mode, stream_for
+from .binding import Operands, PlanBinder, StreamOwner, lo_format, precision_mode, split_mode, stream_for
 from .binding import merge_transposed_weight  # noqa: F401  (callers import it from the generator too)
 
 
@@ -128,10 +128,11 @@ class NetworkBase(StreamOwner, nn.Module):
                 m.__dict__['_lwb_precision'] = mode
 
     def range_flags(self):
-        """-> list of int32[1] device tensors, one per stream used by the most recent pass: bit 0 = an activation left the e4m3 correction
-        range (|x| >= 1024, fp16f8 precision degrades for those elements), bit 1 = the fp16 range (|x| >= 60000 / NaN),
-        bit 2 = output-head pre-activations of +-8 and more in fp16f8 mode (its ~1e-4 relative end-to-end precision then
-        no longer guarantees 1e-3 on the pixels: use fp16x3)."""
+        """-> list of int32[1] device tensors, one per stream used by the most recent pass, with the bits
+        binding.RANGE_F8 = an activation left the e4m3 correction range (|x| >= 1024, fp16f8 precision degrades for those
+        elements), binding.RANGE_FP16 = the fp16 range (|x| >= 60000 / NaN), binding.RANGE_HEADS = output-head
+        pre-activations of +-8 and more in fp16f8 mode (its ~1e-4 relative end-to-end precision then no longer guarantees
+        1e-3 on the pixels: use fp16x3)."""
         live = []
         for m in self.modules():
             for st in getattr(m, '_lwb_streams', {}).values():
@@ -299,7 +300,7 @@ class _Stream(object):
         conv, gamma, beta = layer
         conv.plan.run()
         K.norm_act_nhwc(conv.out, conv.stats, gamma, beta, relu, self.ws, residual=residual, warp_src=warp_src, T=T,
-                        align_corners=ac, y_f32=out.f32, y_hi=out.hi, y_lo=out.lo, lo_format=1 if self.split == 2 else 0,
+                        align_corners=ac, y_f32=out.f32, y_hi=out.hi, y_lo=out.lo, lo_format=lo_format(self.split),
                         range_flag=self.range_flag)
 
     # ---- pieces -------------------------------------------------------------------------
@@ -324,7 +325,7 @@ class _Stream(object):
         if act.f32 is None:
             raise LwbError("second warp needs an fp32 activation")
         K.norm_act_nhwc(act.f32, None, None, None, False, self.ws, warp_src=src, T=T, align_corners=ac,
-                        y_f32=act.f32, y_hi=act.hi, y_lo=act.lo, lo_format=1 if self.split == 2 else 0,
+                        y_f32=act.f32, y_hi=act.hi, y_lo=act.lo, lo_format=lo_format(self.split),
                         range_flag=self.range_flag)
 
     def resnets(self, warp_srcs=None, T=None, ac=False):

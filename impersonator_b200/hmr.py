@@ -23,7 +23,7 @@ import torch.nn as nn
 
 from . import kernels as K
 from ._lib import LwbError
-from .binding import Operands, PlanBinder, StreamOwner, bn_affine, split_mode, stream_for
+from .binding import Operands, PlanBinder, StreamOwner, bn_affine, lo_format, split_mode, stream_for
 from .smpl import SMPL
 
 
@@ -109,7 +109,7 @@ class _HmrStream(object):
 
     def __init__(self, net, B, dev, split):
         self.B, self.dev, self.split = B, dev, split
-        self.lo_format = 1 if split == 2 else 0
+        self.lo_format = lo_format(split)
         r = net.resnet
         self.w1 = r.conv1.weight.detach().float().contiguous()
         self.b1 = r.conv1.bias.detach().float().contiguous()

@@ -31,6 +31,7 @@ import torch
 
 from . import kernels as K
 from ._lib import LwbError
+from .binding import RANGE_F8, RANGE_FP16
 from .generator import ImpersonatorGenerator, weights_epoch
 from .nmr import SMPLRenderer
 
@@ -510,15 +511,15 @@ class Imitator(object):
             self.tsf_info['image'] = last_image[0]
         if range_bits[0] and not getattr(self, '_range_retry', False):
             # Never silently: activations left the range in which the default fp16f8 operand split keeps its precision
-            # (bit 0: |x| >= 1024, the e4m3 correction terms clip; bit 2: output-head pre-activations of +-8 and more, where
-            # its ~1e-4 relative precision may exceed 1e-3 on pixels).  Pin the generator to fp16x3 (fp16 corrections, range
-            # 6e4) and redo the call -- LWB_AUTO_PRECISION=0 only warns; beyond the fp16 range (bit 1) nothing in this
-            # engine can represent the activations.
+            # (RANGE_F8: |x| >= 1024, the e4m3 correction terms clip; RANGE_HEADS: output-head pre-activations of +-8 and
+            # more, where its ~1e-4 relative precision may exceed 1e-3 on pixels).  Pin the generator to fp16x3 (fp16
+            # corrections, range 6e4) and redo the call -- LWB_AUTO_PRECISION=0 only warns; beyond the fp16 range
+            # (RANGE_FP16) nothing in this engine can represent the activations.
             import warnings
-            if range_bits[0] & 2:
+            if range_bits[0] & RANGE_FP16:
                 raise LwbError("generator activations exceed the fp16 range (|x| >= 6e4 or non-finite): the conv engine's "
                                "fp16 operands cannot represent them")
-            what = ("activations beyond the fp16f8 correction range (|x| >= 1024)" if range_bits[0] & 1 else
+            what = ("activations beyond the fp16f8 correction range (|x| >= 1024)" if range_bits[0] & RANGE_F8 else
                     "output-head pre-activations beyond +-8 (fp16f8's ~1e-4 relative precision may exceed 1e-3 on pixels)")
             if os.environ.get("LWB_AUTO_PRECISION", "1") == "0" or getattr(self.generator, '_lwb_precision', None) == "fp16x3" \
                     or os.environ.get("LWB_PRECISION", "fp16f8") != "fp16f8":

@@ -22,7 +22,7 @@ import torch.nn as nn
 
 from . import kernels as K
 from ._lib import LwbError
-from .binding import Operands, PlanBinder, StreamOwner, bn_affine, split_mode, stream_for
+from .binding import Operands, PlanBinder, StreamOwner, bn_affine, lo_format, split_mode, stream_for
 
 
 def get_pad(in_, ksize, stride, atrous=1):
@@ -205,7 +205,7 @@ class _InpaintStream(object):
         if H % 4 or W % 4:
             raise LwbError("InpaintSANet needs H, W divisible by 4")
         self.B, self.H, self.W, self.dev, self.split = B, H, W, dev, split
-        self.lo_format = 1 if split == 2 else 0
+        self.lo_format = lo_format(split)
         self.range_flag = torch.zeros(1, dtype=torch.int32, device=dev)
         self._plans = PlanBinder(dev, split)
         self.in_f32 = torch.zeros((B, H, W, 64), dtype=torch.float32, device=dev)         # channels 4..63 stay zero

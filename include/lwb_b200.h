@@ -23,6 +23,11 @@ extern "C" {
 #define LWB_E_CUDA       -2   /* a CUDA runtime/driver call failed */
 #define LWB_E_UNSUPPORTED -3  /* shape outside what the kernels were built for */
 
+/* Bits of the operand-range flag (the range_flag arguments below) */
+#define LWB_RANGE_F8      1   /* an emitted operand has |y| >= 1024: its e4m3 correction terms clip */
+#define LWB_RANGE_FP16    2   /* an emitted operand has |y| >= 60000 or is not finite: the fp16 hi itself overflows */
+#define LWB_RANGE_HEADS   4   /* a head pre-activation reached +-8 */
+
 typedef void* lwb_stream_t;   /* cudaStream_t */
 
 int         lwb_version(void);
@@ -192,8 +197,9 @@ int lwb_instance_stats_nhwc(const float* x, int n, int h, int w, int c, double* 
  * or a conv bias: networks/hmr.py:66-103).  post_scale / post_shift [c] (nullable): the OPERANDS (y_hi / y_lo) hold
  * relu?(y*post_scale + post_shift) while y_f32 keeps y (pre-activation ResNets: the next block's bn1+relu).
  * res_step s > 1: residual is [n, h*s, w*s, c] and is read at (s*y, s*x) (the subsampled identity shortcut, hmr.py:21-36).
- * range_flag (nullable, device int, caller zero-fills): |= 1 when an emitted operand has |y| >= 1024 (the e4m3 correction
- * terms clip: precision of those elements degrades towards single-pass fp16), |= 2 when |y| >= 60000 or not finite. */
+ * range_flag (nullable, device int, caller zero-fills): |= LWB_RANGE_F8 when an emitted operand has |y| >= 1024 (the e4m3
+ * correction terms clip: precision of those elements degrades towards single-pass fp16), |= LWB_RANGE_F8 | LWB_RANGE_FP16
+ * when |y| >= 60000 or not finite. */
 int lwb_norm_act_nhwc(const float* raw, const double* stats, const float* gamma, const float* beta,
                       float eps, int relu, int n, int h, int w, int c,
                       const float* residual,
@@ -225,7 +231,7 @@ int lwb_glue_kernel_resources(int which, int c, int* out);
  * folded_kw = 0: raw[...,0:4] are the four head channels.  folded_kw = kw (7): raw is the output of the 7x7 heads run on
  * the tensor cores as a kh x 1 filter whose N dimension carries the filter columns, raw[y,x',kx*4+co] (c_stride >= 4*kw);
  * the row sum  out[y,x,co] = sum_kx raw[y, x+kx-kw/2, kx*4+co]  happens here, before tanh / sigmoid.
- * range_flag (nullable, device int): |= 4 when a head pre-activation reaches +-8 -- beyond that the ~1e-4 relative
+ * range_flag (nullable, device int): |= LWB_RANGE_HEADS when a head pre-activation reaches +-8 -- beyond that the ~1e-4 relative
  * end-to-end precision of the split = 2 operand mode no longer guarantees 1e-3 on the pixels (use split = 1). */
 int lwb_heads_composite(const float* raw, int n, int h, int w, int c_stride, int folded_kw,
                         const float* bg, int bg_batch,

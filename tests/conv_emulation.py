@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from impersonator_b200 import kernels as K
+from impersonator_b200.binding import RANGE_F8, RANGE_FP16
 
 # max |got - emulation| / max |emulation|, every operand mode
 EMU_BAR = 3e-5
@@ -34,18 +35,67 @@ def report(name, got, ref):
     return d.max().item() / scale
 
 
+# ------------------------------------------------------------------------------- operand formats (csrc/operands.cuh)
+def fp16_pair(v):
+    """The fp16 hi / lo split of fp32 v: hi = fp16(v), lo = fp16(v - hi)."""
+    hi = v.half()
+    return hi, (v - hi.float()).half()
+
+
+def e4m3(t):
+    """e4m3 with saturation at +-448 (__NV_SATFINITE)."""
+    return t.clamp(-448, 448).to(torch.float8_e4m3fn)
+
+
+def pair_blocks(a, b):
+    """[..., C] e4m3 operands a, b -> [..., 2C] bytes: per 64-channel block, 64 bytes of a then 64 bytes of b."""
+    lead, c = a.shape[:-1], a.shape[-1]
+    blk = torch.stack([e4m3(a).view(torch.uint8).view(*lead, c // 64, 64),
+                       e4m3(b).view(torch.uint8).view(*lead, c // 64, 64)], dim=-2)
+    return blk.reshape(*lead, 2 * c)
+
+
+def act_pair_blocks(v, hi=None):
+    """The activation pair blocks (lo_format 1) of fp32 v [..., C] with its fp16 hi: e4m3(v / 16), e4m3((v - hi) * 1024)."""
+    hi = v.half() if hi is None else hi
+    return pair_blocks(v / 16, (v - hi.float()) * 1024)
+
+
+def range_bits(hi):
+    """The operand-range flag bits of an fp16 hi tensor."""
+    a = hi.float().abs()
+    if bool(((a >= 60000) | torch.isnan(a)).any()):
+        return RANGE_F8 | RANGE_FP16
+    return RANGE_F8 if bool((a >= 1024).any()) else 0
+
+
+# an emitted value, its label and the range bits wanted: fp16 of 1023.7 -> 1023.5, 1023.75 -> 1024 (tie to even),
+# 59983 / 59984 -> 59968 (tie to even), 59990 -> 60000 = 0x7b53, 65520 -> inf
+RANGE_VALUES = (("1023.7", 1023.7, 0), ("1023.75", 1023.75, 1), ("1024", 1024.0, 1), ("-1024", -1024.0, 1),
+                ("59984", 59984.0, 1), ("59990", 59990.0, 3), ("60000", 60000.0, 3), ("65520", 65520.0, 3),
+                ("+inf", float("inf"), 3), ("-inf", float("-inf"), 3), ("nan", float("nan"), 3))
+
+
+def to_f8_operands(cuda, x):
+    """NCHW fp32 -> (hi fp16 NHWC, fp8 pair blocks) through the norm kernel used as a plain converter."""
+    raw = x.permute(0, 2, 3, 1).contiguous().to(cuda)
+    hi = torch.empty(raw.shape, dtype=torch.float16, device=cuda)
+    lo = torch.empty_like(hi)
+    K.norm_act_nhwc(raw, None, None, None, False, None, y_hi=hi, y_lo=lo, lo_format=1)
+    return hi, lo
+
+
+# ------------------------------------------------------------------------------------------------------ emulations
 def split16(v, scale=1.0):
     """(hi, lo) of v * scale as float64 tensors: hi = fp16(v * scale), lo = fp16(v * scale - hi).  v * scale is formed in
     fp32 (exact for a power-of-two scale), like the packers do."""
-    v = v.float() * scale
-    hi = v.half().double()
-    lo = (v.double() - hi).half().double()
-    return hi, lo
+    hi, lo = fp16_pair(v.float() * scale)
+    return hi.double(), lo.double()
 
 
 def q8(t):
     """e4m3 with saturation at +-448 (__NV_SATFINITE), as float64."""
-    return t.clamp(-448, 448).to(torch.float8_e4m3fn).double()
+    return e4m3(t).double()
 
 
 def f8_terms(x, w, conv, w_exp):

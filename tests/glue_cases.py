@@ -18,6 +18,8 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from conv_emulation import RANGE_VALUES, act_pair_blocks, fp16_pair
+
 U32 = 2.0 ** -24               # fp32 unit roundoff
 TAU = 16
 NAN = float("nan")
@@ -130,11 +132,6 @@ def _nhwc(t):
     return t.permute(0, 2, 3, 1)
 
 
-def fp16_pair(v):
-    hi = v.half()
-    return hi, (v - hi.float()).half()
-
-
 def u8_bgr(hwc):
     """cv_utils.save_cv2_img's ((img + 1) / 2.0 * 255).astype(np.uint8) in float32 numpy, channels reversed (RGB2BGR)."""
     a = hwc.numpy().astype(np.float32)
@@ -232,11 +229,7 @@ def _norm_act(edge, seed, n, h, w, c, mode="stats", relu=False, res_step=0, warp
         if lo_format == 0:
             checks.append(Bits("lo", "lo", lambda o: fp16_pair(o["y_f32"])[1]))
         else:
-            def lo8(o):
-                from test_conv_emulation_gpu import pair_blocks
-                v = o["y_f32"]
-                return pair_blocks(v / 16, (v - v.half().float()) * 1024)
-            checks.append(Bits("lo8", lambda o: o["lo"].view(torch.uint8), lo8, kernel_only=True))
+            checks.append(Bits("lo8", lambda o: o["lo"].view(torch.uint8), lambda o: act_pair_blocks(o["y_f32"])))
     else:
         z = y * ps.double() + pt.double()
         if post:
@@ -269,11 +262,7 @@ def norm_act_cases():
                 cases.append(_norm_act("warp sb=%s T %s ac=%d" % (sb, tsize, ac), 310 + 4 * (sb == "n") + 2 * (tsize == "same") + ac,
                                        n, h, w, 32, relu=ac == 0, res_step=1 if sb == "n" else 0,
                                        warp=(1 if sb == "1" else n, th, tw, ac)))
-    # fp16 of the emitted value: 1023.7 -> 1023.5, 1023.75 -> 1024 (tie to even), 59983 / 59984 -> 59968 (tie to even),
-    # 59990 -> 60000 = 0x7b53, 65520 -> inf
-    for label, v, want in (("1023.7", 1023.7, 0), ("1023.75", 1023.75, 1), ("1024", 1024.0, 1), ("-1024", -1024.0, 1),
-                           ("59984", 59984.0, 1), ("59990", 59990.0, 3), ("60000", 60000.0, 3), ("65520", 65520.0, 3),
-                           ("+inf", float("inf"), 3), ("-inf", float("-inf"), 3), ("nan", NAN, 3)):
+    for label, v, want in RANGE_VALUES:
         raw = torch.rand(1, 3, 5, 8, generator=_gen(400)) * 8 - 4
         raw[0, 1, 2, 5] = v
         cases.append(_norm_act("range %s" % label, 400, 1, 3, 5, 8, mode="bare", raw=raw, flag=want))
@@ -820,11 +809,7 @@ def _gated(edge, seed, n, h, w, c, cs, up=1, outputs="f32 hi lo", lo_format=0, b
         if "lo" in outs_on and lo_format == 0:
             checks.append(Bits("lo", "lo", lambda o: _pin_nan(o["lo"], fp16_pair(v_pad(o))[1])))
         elif "lo" in outs_on:
-            def lo8(o):
-                from test_conv_emulation_gpu import pair_blocks
-                v = v_pad(o)
-                return pair_blocks(v / 16, (v - v.half().float()) * 1024)
-            checks.append(Bits("lo8", lambda o: o["lo"].view(torch.uint8), lo8))
+            checks.append(Bits("lo8", lambda o: o["lo"].view(torch.uint8), lambda o: act_pair_blocks(v_pad(o))))
     return Case("gated_act_nhwc", edge, run, checks)
 
 
@@ -859,12 +844,6 @@ INPAINTOR_GATED = [
 
 def _binding_edge(cb):
     return "inpaintor c=%d c_stride=%d up=%d %s lo_format=%d" % cb
-
-
-# fp16 of the emitted value and the bits wanted, as norm_act's range cases
-RANGE_VALUES = (("1023.7", 1023.7, 0), ("1023.75", 1023.75, 1), ("1024", 1024.0, 1), ("-1024", -1024.0, 1),
-                ("59984", 59984.0, 1), ("59990", 59990.0, 3), ("60000", 60000.0, 3), ("65520", 65520.0, 3),
-                ("+inf", float("inf"), 3), ("-inf", float("-inf"), 3), ("nan", NAN, 3))
 
 
 def _gated_range(edge, v, want, outputs="f32 hi lo"):

@@ -9,7 +9,9 @@ works on the fp16 hi/lo operand pairs (run it with LWB_PRECISION=fp16x3); it is 
 import torch
 import torch.nn.functional as F
 
+from conv_emulation import act_pair_blocks, fp16_pair, range_bits
 from impersonator_b200 import kernels as K
+from impersonator_b200.binding import RANGE_HEADS
 
 
 def _pair_to_f32(pair):
@@ -17,16 +19,18 @@ def _pair_to_f32(pair):
     return hi.float() + (lo.float() if lo is not None else 0.0)
 
 
-def _emit(y, y_f32, y_hi, y_lo):
-    if y_f32 is not None:
-        y_f32.copy_(y)
-    if y_hi is not None:
-        c = y.shape[-1]
-        y_hi.zero_()
-        y_hi[..., :c] = y.half()
-        if y_lo is not None:
-            y_lo.zero_()
-            y_lo[..., :c] = (y - y_hi[..., :c].float()).half()
+def _emit(y, y_hi, y_lo, lo_format, range_flag):
+    """y [..., c] -> the operands y_hi / y_lo (nullable) [..., c_pad >= c], channels >= c zero, and the range bits."""
+    v = torch.zeros(y_hi.shape)
+    v[..., :y.shape[-1]] = y
+    hi, lo = fp16_pair(v)
+    y_hi.copy_(hi)
+    if y_lo is not None and lo_format == 1:
+        y_lo.view(torch.uint8).copy_(act_pair_blocks(v, hi))
+    elif y_lo is not None:
+        y_lo.copy_(lo)
+    if range_flag is not None:
+        range_flag |= range_bits(hi)
 
 
 class PackedWeight(tuple):
@@ -132,13 +136,8 @@ def norm_act_nhwc(raw, stats, gamma, beta, relu, ws, eps=1e-5, residual=None, wa
             ops = F.relu(ops)
     if y_f32 is not None:
         y_f32.copy_(v)
-    _emit(ops, None, y_hi, y_lo)
-    if range_flag is not None and y_hi is not None:
-        a = ops.half().float().abs()                # the bits describe the emitted fp16 hi operand
-        if bool(((a >= 60000) | torch.isnan(a)).any()):
-            range_flag |= 3
-        elif bool((a >= 1024).any()):
-            range_flag |= 1
+    if y_hi is not None:
+        _emit(ops, y_hi, y_lo, lo_format, range_flag)
 
 
 def nchw_to_nhwc_split(x, c_pad=None, pad_hw=(0, 0, 0, 0), hi=None, lo=None, split=True):
@@ -150,9 +149,10 @@ def nchw_to_nhwc_split(x, c_pad=None, pad_hw=(0, 0, 0, 0), hi=None, lo=None, spl
     if hi is None:
         hi = torch.empty(full.shape, dtype=torch.float16)
         lo = torch.empty_like(hi) if split else None
-    hi.copy_(full.half())
+    h, l = fp16_pair(full)
+    hi.copy_(h)
     if lo is not None:
-        lo.copy_((full - hi.float()).half())
+        lo.copy_(l)
     return hi, lo
 
 
@@ -194,24 +194,8 @@ def gated_act_nhwc(raw, c, bias, act, scale, shift, upsample=1, clamp=False, y_f
         y = y.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
     if y_f32 is not None:
         y_f32[..., :c] = y                          # columns c.. of a wider f32 buffer are left alone
-    if y_hi is None:
-        return
-    _emit(y, None, y_hi, y_lo if lo_format == 0 else None)
-    if y_lo is not None and lo_format == 1:
-        # the e4m3 pair blocks: per 64 channels, 64 bytes of e4m3(y / 16) then 64 bytes of e4m3((y - hi) * 1024)
-        v = torch.zeros(y_hi.shape)
-        v[..., :c] = y
-        e4m3 = lambda t: t.clamp(-448, 448).to(torch.float8_e4m3fn).view(torch.uint8)      # noqa: E731
-        lead, cp = v.shape[:-1], v.shape[-1]
-        blk = torch.stack([e4m3(v / 16).view(*lead, cp // 64, 64),
-                           e4m3((v - y_hi.float()) * 1024).view(*lead, cp // 64, 64)], dim=-2)
-        y_lo.view(torch.uint8).copy_(blk.reshape(*lead, 2 * cp))
-    if range_flag is not None:
-        a = y_hi.float().abs()                      # the bits describe the emitted fp16 hi operand
-        if bool(((a >= 60000) | torch.isnan(a)).any()):
-            range_flag |= 3
-        elif bool((a >= 1024).any()):
-            range_flag |= 1
+    if y_hi is not None:
+        _emit(y, y_hi, y_lo, lo_format, range_flag)
 
 
 def self_attention_nhwc(qkv, bias, x, gamma, dq=16, out=None):
@@ -302,7 +286,7 @@ def heads_composite(raw, bg=None, want_color=True, want_mask=True, color=None, m
     if pred_u8 is not None:                                  # float32 ((img + 1) / 2.0 * 255) truncated, BGR
         pred_u8.copy_(((p.permute(0, 2, 3, 1) + 1) / 2.0 * 255).to(torch.uint8).flip(-1))
     if range_flag is not None and bool((~(r.abs() < 8)).any()):
-        range_flag |= 4                                      # a pre-activation of magnitude >= 8, or NaN
+        range_flag |= RANGE_HEADS                            # a pre-activation of magnitude >= 8, or NaN
     return tuple(outs)
 
 
@@ -346,10 +330,10 @@ def _store(y, y_f32, y_hi, y_lo, off=0):
     if y_f32 is not None:
         y_f32[..., off:off + c] = y
     if y_hi is not None:
-        hi = y.half()
+        hi, lo = fp16_pair(y)
         y_hi[..., off:off + c] = hi
         if y_lo is not None:
-            y_lo[..., off:off + c] = (y - hi.float()).half()
+            y_lo[..., off:off + c] = lo
 
 
 def det_bias_act(raw, bias=None, relu=False, raw2=None, res=None, res_half=False, step=1, out_hw=None, c=None,

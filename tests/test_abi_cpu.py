@@ -24,6 +24,9 @@ def test_library_exports_every_declared_symbol():
     assert not missing, "declared in include/lwb_b200.h but not exported: %s" % missing
     assert declared == set(_lib.SIGNATURES), (declared ^ set(_lib.SIGNATURES))
     assert L.lwb_version() >= 100
+    from impersonator_b200 import binding
+    bits = dict(re.findall(r"#define LWB_(RANGE_[A-Z0-9]+)\s+(\d+)", header))
+    assert bits and {k: getattr(binding, k) for k in bits} == {k: int(v) for k, v in bits.items()}, bits
 
 
 def test_no_cpu_fallback_when_no_gpu():

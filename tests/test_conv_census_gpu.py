@@ -13,11 +13,10 @@ import pytest
 import torch
 
 import conv_census as C
-from conv_emulation import assert_bands_intact, guarded
+from conv_emulation import assert_bands_intact, guarded, to_f8_operands
 from impersonator_b200 import kernels as K
 from impersonator_b200._lib import ConvDesc
 from impersonator_b200.binding import merge_transposed_weight
-from test_conv_gpu import to_f8_operands
 
 pytestmark = pytest.mark.gpu
 

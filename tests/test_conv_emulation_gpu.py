@@ -15,7 +15,7 @@ import torch
 import torch.nn.functional as F
 
 from impersonator_b200 import kernels as K
-from conv_emulation import assert_bands_intact, check_conv, guarded, report
+from conv_emulation import act_pair_blocks, assert_bands_intact, check_conv, fp16_pair, guarded, pair_blocks, report
 from test_conv_gpu import rnd, run_conv, run_merged_transposed, run_stem
 
 pytestmark = pytest.mark.gpu
@@ -127,22 +127,6 @@ def special_values(shape, seed):
     return v.view(shape).float()
 
 
-def e4m3_bytes(t):
-    return t.clamp(-448, 448).to(torch.float8_e4m3fn).view(torch.uint8)
-
-
-def pair_blocks(a, b):
-    """[..., C] e4m3 operands a, b -> [..., 2C] bytes: per 64-channel block, 64 bytes of a then 64 bytes of b."""
-    lead, c = a.shape[:-1], a.shape[-1]
-    blk = torch.stack([e4m3_bytes(a).view(*lead, c // 64, 64), e4m3_bytes(b).view(*lead, c // 64, 64)], dim=-2)
-    return blk.reshape(*lead, 2 * c)
-
-
-def fp16_pair(v):
-    hi = v.half()
-    return hi, (v - hi.float()).half()
-
-
 def assert_same_bits(name, got, want):
     g, w = got.cpu().contiguous().view(torch.uint8), want.contiguous().view(torch.uint8)
     assert g.shape == w.shape, (name, g.shape, w.shape)
@@ -183,7 +167,7 @@ def test_norm_act_operand_bits(cuda, lo_format):
     if lo_format == 0:
         assert_same_bits("norm_act lo", lo, want_lo)
     else:
-        assert_same_bits("norm_act lo8", lo.view(torch.uint8), pair_blocks(raw / 16, (raw - want_hi.float()) * 1024))
+        assert_same_bits("norm_act lo8", lo.view(torch.uint8), act_pair_blocks(raw, want_hi))
 
 
 def test_gated_act_operand_bits(cuda):
@@ -200,7 +184,7 @@ def test_gated_act_operand_bits(cuda):
     v[..., :c] = y.cpu()
     want_hi, _ = fp16_pair(v)
     assert_same_bits("gated hi", hi, want_hi)
-    assert_same_bits("gated lo8", lo.view(torch.uint8), pair_blocks(v / 16, (v - want_hi.float()) * 1024))
+    assert_same_bits("gated lo8", lo.view(torch.uint8), act_pair_blocks(v, want_hi))
 
 
 def weights(kind, shape, seed):

@@ -7,7 +7,7 @@ import torch
 import torch.nn.functional as F
 
 from impersonator_b200 import kernels as K
-from conv_emulation import check_conv, emulate_f8, report  # noqa: F401  (report, emulate_f8: used by the other conv tests)
+from conv_emulation import check_conv, emulate_f8, report, to_f8_operands  # noqa: F401  (report, emulate_f8: used by the other conv tests)
 
 pytestmark = pytest.mark.gpu
 
@@ -41,15 +41,6 @@ def run_conv(cuda, x, w, stride=1, pad=1, dil=1, transposed=False, split=True, x
     plan.run()
     torch.cuda.synchronize()
     return K.nhwc_to_nchw(out).cpu(), (st.cpu() if st is not None else None), ws.w_exp
-
-
-def to_f8_operands(cuda, x):
-    """NCHW fp32 -> (hi fp16 NHWC, fp8 pair blocks) through the norm kernel used as a plain converter."""
-    raw = x.permute(0, 2, 3, 1).contiguous().to(cuda)
-    hi = torch.empty(raw.shape, dtype=torch.float16, device=cuda)
-    lo = torch.empty_like(hi)
-    K.norm_act_nhwc(raw, None, None, None, False, None, y_hi=hi, y_lo=lo, lo_format=1)
-    return hi, lo
 
 
 CASES = [

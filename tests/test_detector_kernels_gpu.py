@@ -13,6 +13,7 @@ import torch
 import torch.nn.functional as F
 
 import detector_cases as DC
+from conv_emulation import fp16_pair
 from impersonator_b200 import detectors as D, kernels as K, synthetic as S
 from impersonator_b200._lib import LwbError
 from oracle import maskrcnn_ref as R
@@ -40,11 +41,6 @@ def box_ulps(got, want, scale):
     """Box corners: distance in ulps of the coordinate scale each corner was computed at (centre +- half size)."""
     sp = torch.from_numpy(np.spacing(np.abs(scale.float().numpy())).astype(np.float64))
     return float(((got.detach().cpu().double() - want.double()).abs() / sp[:, None]).max()) if want.numel() else 0.0
-
-
-def fp16_pair(v):
-    hi = v.half()
-    return hi, (v - hi.float()).half()
 
 
 def assert_operands(hi, lo, v, what):
