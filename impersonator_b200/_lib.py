@@ -48,6 +48,7 @@ SIGNATURES = {
                                   ctypes.POINTER(_vp)]),
     "lwb_conv_plan_run": (_i, [_vp, _vp]),
     "lwb_conv_plan_num_launches": (_i, [_vp]),
+    "lwb_conv_plan_launch_info": (_i, [_vp, _i, _vp]),
     "lwb_conv_kernel_resources": (_i, [_i, _i, _vp]),
     "lwb_glue_kernel_resources": (_i, [_i, _i, _vp]),
     "lwb_conv_plan_destroy": (None, [_vp]),

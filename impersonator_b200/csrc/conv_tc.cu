@@ -47,7 +47,8 @@
 //   concat input  : K chunks 0..chunks0-1 from tensor 0, the rest from tensor 1 (torch.cat free)
 //   7x7 stem      : "row-K" trick -- with 8 channels per pixel, 8 consecutive pixels of a padded
 //                   NHWC8 row are 64 contiguous fp16, so one K = 64 stage covers a whole filter
-//                   row (overlapping-stride tensor map); 7 stages instead of 49.
+//                   row (overlapping-stride tensor map); 7 stages instead of 49.  With 16 or 24 channels per
+//                   pixel (the wide conditioning maps) a filter row is 2 or 3 such K stages.
 // Epilogue: accumulator registers -> fp32 NHWC global + per-(n, c) sum / sum of squares for the
 // InstanceNorm that follows every conv (f64 atomics).
 #include <cuda.h>
@@ -731,6 +732,9 @@ struct lwb_conv_plan {
     Launch launches[4];
 };
 
+// Padded channels per pixel of a row-K stem input: 8 (one K stage per filter row), 16 or 24 (two or three).
+static bool rowk_cin(int cin0) { return cin0 == 8 || cin0 == 16 || cin0 == 24; }
+
 // NHWC activation view of every step-th pixel from (py, px): element (y', x') = input (step y' + py, step x' + px).
 // step 1 is the plain view, step 2 the parity views of stride-2 convs.
 static View nhwc_view(const uint16_t* hi, const uint16_t* lo, int n, int h, int w, int c, int step = 1, int py = 0, int px = 0)
@@ -848,7 +852,7 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     if (d->halo) {
         // halo plans ("same"-padded stride-1 k x k convs and the row-K stem) run through the tap-group kernel below
         LWB_CHECK_ARG(d->stride == 1 && !d->transposed && d->dil == 1, "halo mode needs stride 1, dilation 1, not transposed");
-        if (d->rowk) LWB_CHECK_ARG(d->kw <= 8 && d->cin0 == 8 && d->cin1 == 0 && d->row_pitch >= d->w_in + 8, "row-K shape");
+        if (d->rowk) LWB_CHECK_ARG(d->kw <= 8 && rowk_cin(d->cin0) && d->cin1 == 0 && d->row_pitch >= d->w_in + 8, "row-K shape");
         else         LWB_CHECK_ARG(d->kw <= 9 && (d->kw & 1) && (d->kh & 1), "halo mode needs an odd kernel, kw <= 9, with 'same' padding (kh/2, kw/2)");
     }
 
@@ -863,16 +867,21 @@ extern "C" int lwb_conv_plan_create(const lwb_conv_desc* d,
     LaunchSpec specs[4];
     int num = 1;
     if (d->rowk) {
-        // 7x7 stem through the row-K trick.  Input: padded NHWC8 buffer [n, h_in + kh - 1, wp, 8] whose
-        // pixel (y + pad, x + pad) holds input pixel (y, x); wp >= w_in + 8.  One K = 64 stage = 8
-        // consecutive pixels x 8 channels of a padded row = one whole filter row (8th tap weight = 0).
-        LWB_CHECK_ARG(d->stride == 1 && !d->transposed && d->kw <= 8 && d->cin0 == 8 && d->cin1 == 0, "row-K needs stride 1, kw <= 8, 8 channels");
+        // 7x7 stem through the row-K trick.  Input: padded NHWC buffer [n, h_in + kh - 1, wp, cpx] (cpx = cin0 = 8, 16
+        // or 24 channels per pixel) whose pixel (y + pad, x + pad) holds input pixel (y, x); wp >= w_in + 8.  8
+        // consecutive pixels of a padded row are 8 cpx contiguous fp16 = one whole filter row (taps kx >= kw weigh 0):
+        // K = 8 cpx per filter row, in cpx / 8 stages of 64.  The activation view steps one pixel (cpx elements) per
+        // output column and spans 8 cpx elements, so stage c of output pixel x reads pixels x + 8c/cpx ..; the packed
+        // weights [ky][cout][kx * cpx + c] (lwb_pack_conv_weight_rowk, cpx) follow the same K order.
+        LWB_CHECK_ARG(d->stride == 1 && !d->transposed && d->kw <= 8, "row-K needs stride 1, kw <= 8, 8 channels");
+        LWB_CHECK_ARG(rowk_cin(d->cin0) && d->cin1 == 0, "row-K needs 8, 16 or 24 padded input channels in one input");
         LWB_CHECK_ARG(d->h_out == d->h_in && d->w_out == d->w_in && d->row_pitch >= d->w_in + 8, "row-K shape");
         for (int ky = 0; ky < d->kh; ky++) s.tap(ky, 0, 0, ky);
-        s.chunks0 = 1;
-        const uint64_t hp = d->h_in + d->kh - 1, row_bytes = (uint64_t)d->row_pitch * 16;
-        s.a[0] = View{x0_hi, x0_lo, {64, (uint64_t)d->w_in, hp, (uint64_t)d->n}, {16, row_bytes, hp * row_bytes}};
-        s.w = weight_view(w_hi, w_lo, 64, d->cout, d->kh);
+        const int k_row = 8 * d->cin0;                       // K of one filter row
+        s.chunks0 = k_row / KCHUNK;
+        const uint64_t hp = d->h_in + d->kh - 1, px_bytes = (uint64_t)d->cin0 * 2, row_bytes = (uint64_t)d->row_pitch * px_bytes;
+        s.a[0] = View{x0_hi, x0_lo, {(uint64_t)k_row, (uint64_t)d->w_in, hp, (uint64_t)d->n}, {px_bytes, row_bytes, hp * row_bytes}};
+        s.w = weight_view(w_hi, w_lo, k_row, d->cout, d->kh);
     } else {
         LWB_CHECK_ARG(d->cin0 % KCHUNK == 0 && d->cin1 % KCHUNK == 0 && d->cin0 > 0, "input channels must be multiples of 64");
         LWB_CHECK_ARG(d->cin1 == 0 || (x1_hi && (!split || x1_lo)), "second input missing");
@@ -957,6 +966,15 @@ extern "C" int lwb_conv_plan_run(const lwb_conv_plan* plan, lwb_stream_t stream)
 extern "C" void lwb_conv_plan_destroy(lwb_conv_plan* plan) { delete plan; }
 
 extern "C" int lwb_conv_plan_num_launches(const lwb_conv_plan* plan) { return plan ? plan->num : 0; }
+
+extern "C" int lwb_conv_plan_launch_info(const lwb_conv_plan* plan, int i, int* out)
+{
+    LWB_CHECK_ARG(plan && out, "null pointer");
+    LWB_CHECK_ARG(i >= 0 && i < plan->num, "launch index out of range");
+    const Launch& L = plan->launches[i];
+    out[0] = L.n_tile; out[1] = L.mode; out[2] = L.p.chunks0 + L.p.chunks1; out[3] = L.p.ntaps;
+    return LWB_OK;
+}
 
 extern "C" int lwb_conv2d_nhwc(const lwb_conv_desc* d,
                                const uint16_t* x0_hi, const uint16_t* x0_lo,

@@ -79,6 +79,17 @@ def fold_head_weights(w_img, w_att):
     return torch.cat([folded, torch.zeros(4, w4.shape[1], 7, 1, dtype=folded.dtype, device=folded.device)], dim=0).contiguous()
 
 
+STEM_MAX_CIN = 24                                          # input channels the row-K stem takes (3 + the widest map, 15)
+
+
+def stem_cin_pad(cin):
+    """Channels per pixel of the stem's padded input for ``cin`` input channels: 8 (one K stage of 64 per filter row),
+    16 or 24 (two or three stages): the 3 + cond channels of every map of mesh.get_map_fn_dim fit."""
+    if not 0 < cin <= STEM_MAX_CIN:
+        raise LwbError("the 7x7 stem takes 1 to %d input channels, not %d" % (STEM_MAX_CIN, cin))
+    return (cin + 7) // 8 * 8
+
+
 def _halo_mode():
     """LWB_HALO: '0' (default) = CUDA-core 7x7 heads; 'auto' = halo plans for the row-K stem and the skippers + 7x7
     heads on tensor cores (N tile 16); 'all' = also the residual blocks.  Halo plans run through the same tap-group conv
@@ -208,8 +219,7 @@ class _Stream(object):
         if H % (1 << nd) or W % (1 << nd):
             raise LwbError("image size must be divisible by %d" % (1 << nd))
         self.cin = enc[0][0].weight.shape[1]
-        if self.cin > 8:
-            raise LwbError("stem supports at most 8 input channels")
+        self.cin_pad = stem_cin_pad(self.cin)
         # InstanceNorm statistics of every conv + the operand-range flag share one buffer: one fill per pass
         norms = [m for m in net.modules() if isinstance(m, nn.InstanceNorm2d)]
         cmax = max([16] + [m.num_features for m in norms])
@@ -232,10 +242,10 @@ class _Stream(object):
         c0 = enc[0][0].weight.shape[0]
         tc = _tc_heads() and c0 == 64                            # folded heads, unless the halo heads run
         heads_tc = hm != '0' or tc                                # the heads read fp16 operands, else fp32
-        # stem input: padded NHWC8 (3 px border top/left/bottom, 5 right) for the row-K 7x7 conv, which keeps the fp16
-        # hi/lo input
-        self.x_pad = Operands((B, H + 6, W + 8, 8), dev, split)
-        self.enc_layers = [conv_norm(*enc[0], self.x_pad.pair, H, W, rowk=True, row_pitch=W + 8, cin_pad=8,
+        # stem input: padded NHWC of 8, 16 or 24 channels (3 px border top/left/bottom, 5 right) for the row-K 7x7 conv,
+        # which keeps the fp16 hi/lo input
+        self.x_pad = Operands((B, H + 6, W + 8, self.cin_pad), dev, split)
+        self.enc_layers = [conv_norm(*enc[0], self.x_pad.pair, H, W, rowk=True, row_pitch=W + 8, cin_pad=self.cin_pad,
                                      split=min(split, 1), halo=(hm != '0'))]
         c, h, w = c0, H, W
         self.e = [Operands((B, h, w, c), dev, split, f32=keep_f32)]
@@ -307,7 +317,7 @@ class _Stream(object):
     def load_input(self, x):
         if tuple(x.shape) != (self.B, self.cin, self.H, self.W) or x.dtype != torch.float32:
             raise LwbError("unexpected input %s (stream built for %s)" % (tuple(x.shape), (self.B, self.cin, self.H, self.W)))
-        K.nchw_to_nhwc_split(x.contiguous(), c_pad=8, pad_hw=(3, 3, 3, 5), hi=self.x_pad.hi, lo=self.x_pad.lo)
+        K.nchw_to_nhwc_split(x.contiguous(), c_pad=self.cin_pad, pad_hw=(3, 3, 3, 5), hi=self.x_pad.hi, lo=self.x_pad.lo)
 
     def encode(self, warp_srcs=None, T=None, ac=False):
         """encoders 0..n_down; warp_srcs[i] (NHWC fp32, i >= 1) is LWB-added after encoder i."""

@@ -129,8 +129,13 @@ class Imitator(object):
         else:
             self.hmr = self._create_hmr().to(self.device).eval()
         if render is None:
+            # the conditioning table follows --map_name (mesh.create_mapping), so it matches the generator's input width
             render = SMPLRenderer(image_size=opt.image_size, tex_size=getattr(opt, 'tex_size', 3),
+                                  map_name=getattr(opt, 'map_name', '') or 'uv_seg',
                                   has_front=getattr(opt, 'front_warp', False), fill_back=False)
+            if render.map_fn.shape[1] != self._G_cond_nc:
+                raise LwbError("the '%s' table has %d columns, the generator is conditioned on %d channels"
+                               % (render.map_name, render.map_fn.shape[1], self._G_cond_nc))
         self.render = render.to(self.device)
         if detector is not None:
             self.detector = detector

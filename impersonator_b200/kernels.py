@@ -307,6 +307,13 @@ class ConvPlan(object):
 
     prof_class = "conv"                  # instrumentation class (bench.py breakdown); the folded heads report as "heads"
 
+    def launch_info(self, i=0):
+        """-> dict(n_tile, mode, k_stages, taps) of launch i (lwb_conv_plan_launch_info): the kernel instance is
+        (n_tile, mode); k_stages = K stages of 64 per filter tap."""
+        out = (ctypes.c_int * 4)()
+        check(lib().lwb_conv_plan_launch_info(self._h, i, out), "lwb_conv_plan_launch_info")
+        return dict(zip(("n_tile", "mode", "k_stages", "taps"), out))
+
     def run(self):
         _count(self.num_launches)
         with _Prof(self.prof_class, self.flops, self.label):

@@ -112,9 +112,13 @@ def create_mapping(map_name, mapping_path='assets/pretrains/mapper.txt', part_in
     elif map_name == 'back':
         map_fn, bg = _mask(nf, set(_face_set(head_info)) - set(_face_set(front_info)), fill_back)
     elif map_name == 'ids':
-        map_fn, bg = np.arange(0, 1, 1 / nf, dtype=np.float32), np.array([[-1]], dtype=np.float32)
+        # one column (the reference's 1-D arange cannot be stacked on its [1, 1] background row); np.arange with a float
+        # step may return nf + 1 values
+        map_fn, bg = np.arange(0, 1, 1 / nf, dtype=np.float32)[:nf, None], np.array([[-1]], dtype=np.float32)
     elif map_name == 'binary':
-        width = len(np.binary_repr(nf))
+        # the face index in at least get_map_fn_dim('binary') = 15 bits, the width the generator is built for (the
+        # reference codes it in len(binary_repr(nf)) bits: 14 for the 13776 SMPL faces, one column short of its generator)
+        width = max(len(np.binary_repr(nf)), get_map_fn_dim('binary'))
         map_fn = np.stack([np.array(list(map(int, np.binary_repr(i, width=width)))) for i in range(nf)], axis=0)
         bg = np.zeros((1, width), dtype=np.float32) - 1.0
     else:

@@ -166,12 +166,13 @@ def synthetic_flow(batch, image_size=256, seed=5):
     return T
 
 
-def synthetic_generator_inputs(batch, image_size=256, seed=11):
-    """-> dict(bg f32[1,4,H,W], src f32[1,6,H,W], tsf f32[B,6,H,W], T f32[B,H,W,2]) in [-1,1]."""
+def synthetic_generator_inputs(batch, image_size=256, seed=11, cin=6):
+    """-> dict(bg f32[1,4,H,W], src f32[1,cin,H,W], tsf f32[B,cin,H,W], T f32[B,H,W,2]) in [-1,1]; cin = 3 + the
+    conditioning channels of the map (6 for uv_seg, 14 for par, 18 for binary)."""
     g = torch.Generator().manual_seed(seed)
     r = lambda *s: torch.rand(*s, generator=g) * 2 - 1
-    return dict(bg=r(1, 4, image_size, image_size), src=r(1, 6, image_size, image_size),
-                tsf=r(batch, 6, image_size, image_size), T=synthetic_flow(batch, image_size, seed + 1))
+    return dict(bg=r(1, 4, image_size, image_size), src=r(1, cin, image_size, image_size),
+                tsf=r(batch, cin, image_size, image_size), T=synthetic_flow(batch, image_size, seed + 1))
 
 
 # SMPL kinematic tree (kintree_table[0] of the public SMPL model; entry 0 is the root, stored as uint32 -1)

@@ -146,7 +146,8 @@ typedef struct lwb_conv_desc {
                                  an ordinary OIHW [4*cout, cin, 2, 2] filter; cout % 32 == 0, cout <= 128 recommended */
     int split;                /* 1 = 3-pass fp16 split (parity mode), 0 = single pass ("fast"), 2 = fp16 main product +
                                  both small products in fp8 (lo operands from lwb_pack_conv_weight_f8 / lo_format 1) */
-    int rowk;                 /* 1 = 7x7-stem row-K mode: input is a padded NHWC8 buffer (see conv_tc.cu) */
+    int rowk;                 /* 1 = 7x7-stem row-K mode: input is a padded NHWC buffer of cin0 = 8, 16 or 24 channels
+                                 (see conv_tc.cu), weights from lwb_pack_conv_weight_rowk with cpx = cin0, kxs = 8 */
     int row_pitch;            /* rowk: pixels per padded row (>= w_in + 8) */
     int n_tile;               /* 0 = auto; else force the N tile (16/32/64/128, must divide cout; 256 runs as 128) */
     int halo;                 /* 1 = halo plan (stride-1 'same' k x k convs and the row-K stem): checked as such, then run
@@ -168,6 +169,9 @@ int  lwb_conv_plan_create(const lwb_conv_desc* d,
                           float* out_raw, double* stats, lwb_conv_plan** plan);
 int  lwb_conv_plan_run(const lwb_conv_plan* plan, lwb_stream_t stream);
 int  lwb_conv_plan_num_launches(const lwb_conv_plan* plan);
+/* The kernel instance and K loop of launch i of a plan: out[4] = {N tile, operand mode, K stages of 64 per filter tap,
+ * filter taps}.  A row-K stem over 8 / 16 / 24 padded channels has 1 / 2 / 3 K stages per tap (one tap per filter row). */
+int  lwb_conv_plan_launch_info(const lwb_conv_plan* plan, int i, int* out);
 void lwb_conv_plan_destroy(lwb_conv_plan* plan);
 /* Resources of the conv kernel instance (n_tile 16/32/64/128, mode = lwb_conv_desc.split) as launched:
  * out[7] = {registers per thread at launch, static smem, dynamic smem, local bytes per thread, threads per CTA,
