@@ -60,6 +60,7 @@ SIGNATURES = {
     "lwb_conv7x7_heads_nhwc": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "lwb_heads_composite": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lwb_frames_out": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
+    "lwb_frames_in": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, _vp]),
     "lwb_gated_bn_nchw": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "lwb_smpl_workspace_bytes": (_sz, [_i]),
     "lwb_smpl_forward": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i,

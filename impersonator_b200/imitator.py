@@ -81,6 +81,23 @@ def _save_image(img, path, image_size=None, normalize=False):
     cv2.imwrite(path, img)
 
 
+def _frame_stack(frames):
+    """Target frames as one uint8 [N,H,W,3] array or tensor (a sequence of [H,W,3] frames is stacked; they must share a
+    size)."""
+    if not (torch.is_tensor(frames) or isinstance(frames, np.ndarray)):
+        frames = list(frames)
+        if not frames:
+            return np.zeros((0, 1, 1, 3), np.uint8)
+        shapes = {tuple(f.shape) for f in frames}
+        if len(shapes) != 1:
+            raise LwbError("tgt_frames differ in size (%s): one call takes frames of one size" % sorted(shapes))
+        frames = torch.stack([torch.as_tensor(f) for f in frames]) if torch.is_tensor(frames[0]) else np.stack(frames)
+    u8 = frames.dtype == torch.uint8 if torch.is_tensor(frames) else frames.dtype == np.uint8
+    if not u8 or frames.ndim != 4 or frames.shape[3] != 3:
+        raise LwbError("tgt_frames must be uint8 [N,H,W,3], got %s %s" % (frames.dtype, tuple(frames.shape)))
+    return frames.contiguous() if torch.is_tensor(frames) else np.ascontiguousarray(frames)
+
+
 class Imitator(object):
     """``Imitator(opt)`` builds everything from ``opt`` exactly like models/imitator.py:15-74 (+ models/models.py:64-76,
     159-179): generator through ``NetworksFactory`` + checkpoint, background net, HMR (+ SMPL), ``SMPLRenderer`` from the
@@ -205,8 +222,11 @@ class Imitator(object):
     # ---- personalize (models/imitator.py:82-145) ----------------------------------------------
     @_on_device
     @torch.no_grad()
-    def personalize(self, src_path, src_smpl=None, output_path='', visualizer=None, src_img=None):
-        self.src_info = self._personalize(src_path, src_smpl, output_path, visualizer, src_img)
+    def personalize(self, src_path, src_smpl=None, output_path='', visualizer=None, src_img=None, src_frame=None):
+        """models/imitator.py:82-145.  ``src_frame`` (extension): one uint8 frame [H,W,3], B,G,R as cv2.imread returns it,
+        on the host or the device, in place of the file at ``src_path`` (which may then be '').  It is resized on the
+        device exactly as the file would be (kernels.frames_in), and ``src_info['image']`` keeps it as given."""
+        self.src_info = self._personalize(src_path, src_smpl, output_path, visualizer, src_img, src_frame)
         self.__dict__['_graphs'] = {}                    # captured chunk graphs hold the previous source's buffers
 
     def _original_bg(self, bg_inputs, img_bg):
@@ -217,10 +237,17 @@ class Imitator(object):
     def _extend_src_info(self, src_info):
         """Task-specific additions to ``src_info`` (models/swapper.py:128-129 adds the part map)."""
 
-    def _personalize(self, src_path, src_smpl=None, output_path='', visualizer=None, src_img=None):
+    def _personalize(self, src_path, src_smpl=None, output_path='', visualizer=None, src_img=None, src_frame=None):
         """The body shared by models/imitator.py:82-145, models/viewer.py:83-143 and models/swapper.py:99-165 -> src_info."""
         size = self._opt.image_size
-        if src_img is None:
+        img_hmr = gt_u8 = None
+        if src_frame is not None:
+            if src_img is not None:
+                raise LwbError("give the source as src_img or as src_frame, not both")
+            img, img_hmr, gt_u8 = K.frames_in(src_frame, size, want_hmr=src_smpl is None and self.hmr is not None,
+                                              want_u8=bool(output_path))
+            ori_img = src_frame
+        elif src_img is None:
             img, ori_img = _read_image(src_path, size)
             img = torch.tensor(img * 2 - 1.0, dtype=torch.float32, device=self.device)[None, ...]
         else:
@@ -228,9 +255,11 @@ class Imitator(object):
         if src_smpl is None:
             if self.hmr is None or ori_img is None:
                 raise LwbError("src_smpl required when no HMR network is injected")
-            import cv2
-            img_hmr = cv2.resize(ori_img, (224, 224)).astype(np.float32).transpose((2, 0, 1)) / 255.0 * 2 - 1.0
-            src_smpl = self.hmr(torch.tensor(img_hmr, dtype=torch.float32, device=self.device)[None, ...])
+            if img_hmr is None:
+                import cv2
+                img_hmr = cv2.resize(ori_img, (224, 224)).astype(np.float32).transpose((2, 0, 1)) / 255.0 * 2 - 1.0
+                img_hmr = torch.tensor(img_hmr, dtype=torch.float32, device=self.device)[None, ...]
+            src_smpl = self.hmr(img_hmr)
         else:
             src_smpl = torch.as_tensor(src_smpl, dtype=torch.float32, device=self.device).reshape(1, -1)
 
@@ -267,7 +296,10 @@ class Imitator(object):
         if visualizer is not None:
             visualizer.vis_named_img('src', img)
             visualizer.vis_named_img('bg', src_info['bg'])
-        if output_path and ori_img is not None:
+        if output_path and gt_u8 is not None:
+            import cv2
+            cv2.imwrite(output_path, gt_u8[0].cpu().numpy())
+        elif output_path and ori_img is not None:
             _save_image(ori_img, output_path, image_size=size)
         return src_info
 
@@ -415,7 +447,7 @@ class Imitator(object):
     @_on_device
     @torch.no_grad()
     def inference(self, tgt_paths, tgt_smpls=None, cam_strategy='smooth', output_dir='', visualizer=None, verbose=True,
-                  as_uint8=False, score_against=None, lpips=None):
+                  as_uint8=False, score_against=None, lpips=None, tgt_frames=None):
         """models/imitator.py:157-189.  Returns per-frame float32 HxWx3 arrays in [-1,1] like the reference; with
         ``as_uint8=True`` (extra) returns the BGR uint8 images the reference writes to disk instead (4x less D2H).
         With ``output_dir`` the uint8 images come from the GPU and go straight to cv2.imwrite.
@@ -423,7 +455,20 @@ class Imitator(object):
         ``score_against`` (extra): ground-truth frames [N,3,H,W] in [-1,1] (numpy or tensor, N = len(tgt_paths)).  Each
         chunk's frames are scored while still on the device (impersonator_b200.metrics.score_frames: SSIM and PSNR, and
         LPIPS when an ``lpips`` = metrics.LPIPS is given), and the call returns (outputs, scores) with scores a dict of
-        per-frame float64 numpy arrays."""
+        per-frame float64 numpy arrays.
+
+        ``tgt_frames`` (extension): the target frames themselves instead of files -- uint8 [N,H,W,3], B,G,R as cv2.imread
+        returns them, a numpy array or a tensor on the host or the device, or a sequence of [H,W,3] frames of one size.
+        ``tgt_paths`` must then be empty or all ''.  Each chunk's frames are resized on the device in one launch
+        (kernels.frames_in) into the HMR input and, with ``output_dir``, the gt_ images, byte for byte what the file route
+        computes; a host source is uploaded on the copy stream one chunk ahead.  ``tsf_info['image']`` is the last frame
+        as given; the files are named like inference_by_smpls names them (gt_%.8d.jpg beside pred_%.8d.jpg)."""
+        if tgt_frames is not None:
+            tgt_frames = _frame_stack(tgt_frames)
+            if tgt_paths and (any(tgt_paths) or len(tgt_paths) != len(tgt_frames)):
+                raise LwbError("tgt_paths and tgt_frames both name the target frames: give tgt_paths as [] (or "
+                               "%d empty strings) with tgt_frames" % len(tgt_frames))
+            tgt_paths = [''] * len(tgt_frames)
         length = len(tgt_paths)
         if score_against is not None:
             from . import metrics as _metrics
@@ -434,9 +479,24 @@ class Imitator(object):
         last_image = [None]
         originals = {}                                           # frame index -> original RGB image (for the gt_ files)
 
+        frame_u8 = {}                                            # chunk start -> its gt_ images, BGR uint8 on the device
+
         def chunk_smpls(a, b):
             """SMPL vectors of frames a..b-1: given, or estimated from the target images by HMR -- one encoder batch per
             chunk instead of one launch sequence per frame (models/imitator.py:271-275)."""
+            if tgt_frames is not None:
+                want_hmr = tgt_smpls is None
+                if want_hmr and (self.hmr is None or not callable(self.hmr)):
+                    raise LwbError("tgt_smpls required when no HMR network is available")
+                last_image[0] = tgt_frames[b - 1]
+                if want_hmr or output_dir:
+                    _, hmr_in, gt = K.frames_in(chunk_frames(a, b), self._opt.image_size, want_img=False,
+                                                want_hmr=want_hmr, want_u8=bool(output_dir))
+                    if gt is not None:
+                        frame_u8[a] = gt
+                if not want_hmr:
+                    return torch.as_tensor(np.stack([np.asarray(s, dtype=np.float32).reshape(-1) for s in tgt_smpls[a:b]]))
+                return self.hmr(hmr_in)
             if tgt_smpls is not None:
                 return torch.as_tensor(np.stack([np.asarray(s, dtype=np.float32).reshape(-1) for s in tgt_smpls[a:b]]))
             if self.hmr is None or not callable(self.hmr):
@@ -457,10 +517,33 @@ class Imitator(object):
             self._copy_stream = torch.cuda.Stream(device=self.device)
         pending = []
         range_bits = [0]
+        uploads = {}                                             # chunk start -> (frames on the device, copy finished)
+        host_frames = tgt_frames is not None and not (torch.is_tensor(tgt_frames) and tgt_frames.is_cuda)
+
+        def upload(a, b):
+            """H2D of a host chunk on the copy stream (two staging slots: one chunk in flight while the next is filled)."""
+            with torch.cuda.stream(self._copy_stream):
+                dev = K.upload_u8(tgt_frames[a:b], self.device, slot=chunks.index((a, b)) % 2)
+                done = torch.cuda.Event()
+                done.record(self._copy_stream)
+            dev.record_stream(main)
+            uploads[a] = (dev, done)
+
+        def chunk_frames(a, b):
+            if not host_frames:
+                return tgt_frames[a:b]
+            if a not in uploads:
+                upload(a, b)
+            dev, done = uploads.pop(a)
+            main.wait_event(done)
+            nxt = [(c, d) for (c, d) in chunks if c == b]
+            if nxt:
+                upload(*nxt[0])                                  # overlaps this chunk's generator pass
+            return dev
 
         def drain(keep):
             while len(pending) > keep:
-                a0, b0, h_f, h_u8, h_flag, done = pending.pop(0)
+                a0, b0, h_f, h_u8, h_gt, h_flag, done = pending.pop(0)
                 done.synchronize()
                 if h_flag is not None:
                     range_bits[0] |= int(h_flag[0])
@@ -469,9 +552,11 @@ class Imitator(object):
                     outputs.append(host[j])
                     if output_dir:
                         self._maybe_save(h_u8[j], tgt_paths[a0 + j], output_dir, a0 + j, is_bgr_u8=True,
-                                         original=originals.pop(a0 + j, None))
+                                         original=originals.pop(a0 + j, None),
+                                         gt_u8=h_gt[j] if h_gt is not None else None)
 
-        for (a, b) in self._chunks(length):
+        chunks = self._chunks(length)
+        for (a, b) in chunks:
             smpls = torch.as_tensor(chunk_smpls(a, b), dtype=torch.float32).to(self.device, non_blocking=True)
             if smpls.dim() == 1:
                 smpls = smpls[None, ...]
@@ -492,12 +577,14 @@ class Imitator(object):
                 h_f = self._to_host(out_hwc, sync=False) if not as_uint8 else None
                 h_u8 = self._to_host(out_u8, sync=False) if want_u8 else None
                 h_flag = self._to_host(flag, sync=False) if flag is not None else None
-                for t in (out_hwc, out_u8, flag):
+                gt = frame_u8.pop(a, None)
+                h_gt = self._to_host(gt, sync=False) if gt is not None else None
+                for t in (out_hwc, out_u8, flag, gt):
                     if t is not None:
                         t.record_stream(self._copy_stream)
                 done = torch.cuda.Event()
                 done.record(self._copy_stream)
-            pending.append((a, b, h_f, h_u8, h_flag, done))
+            pending.append((a, b, h_f, h_u8, h_gt, h_flag, done))
             drain(keep=1)
         drain(keep=0)
 
@@ -538,7 +625,7 @@ class Imitator(object):
                 if enc_in is not None:
                     self.src_info['feats'] = self.generator.encode_src(enc_in)
                 return self.inference(tgt_paths, tgt_smpls, cam_strategy, output_dir, visualizer, verbose, as_uint8,
-                                      score_against, lpips)
+                                      score_against, lpips, tgt_frames)
             finally:
                 self._range_retry = False
         return result()
@@ -567,14 +654,18 @@ class Imitator(object):
                 info[k] = v[-1:].clone()                 # own storage: the chunk buffers may belong to a replayed graph
         self.tsf_info = info
 
-    def _maybe_save(self, pred, tgt_path, output_dir, t, is_bgr_u8=False, original=None):
+    def _maybe_save(self, pred, tgt_path, output_dir, t, is_bgr_u8=False, original=None, gt_u8=None):
         """pred_<file> (+ gt_<file> = the driving frame resized, models/imitator.py:182-187); inference_by_smpls names
-        its frames pred_%.8d.jpg (:212)."""
+        its frames pred_%.8d.jpg (:212).  ``gt_u8``: the driving frame already resized (BGR uint8), written as
+        gt_<file>, or gt_%.8d.jpg where there is no file name."""
         if not output_dir:
             return
         name = os.path.split(tgt_path)[-1] if tgt_path else 'pred_%.8d.jpg' % t
         path = os.path.join(output_dir, 'pred_' + name if tgt_path else name)
-        if tgt_path:
+        if gt_u8 is not None:
+            import cv2
+            cv2.imwrite(os.path.join(output_dir, 'gt_' + name if tgt_path else 'gt_%.8d.jpg' % t), gt_u8)
+        elif tgt_path:
             if original is None:
                 _, original = _read_image(tgt_path, self._opt.image_size)
             _save_image(original, os.path.join(output_dir, 'gt_' + name), image_size=self._opt.image_size)

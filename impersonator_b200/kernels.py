@@ -479,6 +479,60 @@ def frames_out(frames, want_hwc=True, want_u8=False):
     return hwc, u8
 
 
+_staging = {}              # (device index, slot) -> (pinned uint8 buffer, event recorded after its last H2D copy)
+
+
+def upload_u8(frames, device=None, slot=0):
+    """A host uint8 array / tensor -> the same uint8 tensor on ``device`` (default: the current one), copied on the current
+    stream through a pinned staging buffer that is reused from call to call (per device and ``slot``: a caller that keeps
+    two uploads in flight uses two slots).  Waits only for the previous copy out of the same buffer."""
+    a = frames.numpy() if torch.is_tensor(frames) else np.asarray(frames)
+    if a.dtype != np.uint8:
+        raise LwbError("frames must be uint8, got %s" % a.dtype)
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    key = (device.index, slot)
+    buf, done = _staging.get(key, (None, None))
+    if done is not None:
+        done.synchronize()
+    if buf is None or buf.numel() < a.size:
+        buf = torch.empty(max(a.size, 1), dtype=torch.uint8, pin_memory=True)
+    np.copyto(buf.numpy()[:a.size].reshape(a.shape), a)
+    out = torch.empty(a.shape, dtype=torch.uint8, device=device)
+    out.view(-1).copy_(buf[:a.size], non_blocking=True)
+    done = torch.cuda.Event()
+    done.record(torch.cuda.current_stream(device))
+    _staging[key] = (buf, done)
+    return out
+
+
+def frames_in(frames, size, hmr_size=224, bgr=True, want_img=True, want_hmr=True, want_u8=False):
+    """uint8 frames [n,H,W,3] or [H,W,3] (a CUDA tensor, or a host array / tensor, uploaded with ``upload_u8``), B,G,R
+    as cv2.imread returns them (``bgr=False``: R,G,B) -> (img, hmr, u8), each None unless asked for:
+
+      img  fp32 [n,3,size,size] RGB in [-1,1]: cv2.resize(rgb, (size, size)) / 255.0 * 2 - 1.0 (utils/cv_utils.py:10-47)
+      hmr  fp32 [n,3,hmr_size,hmr_size] RGB in [-1,1]: the same from the frame itself (the HMR input)
+      u8   uint8 [n,size,size,3] BGR: what cv_utils.save_cv2_img(frame, image_size=size) writes
+
+    One kernel launch (lwb_frames_in); every byte equals cv2.resize's uint8 INTER_LINEAR result on the same frame."""
+    if not torch.is_tensor(frames) or not frames.is_cuda:
+        frames = upload_u8(frames)
+    _chk_cuda(frames)
+    if frames.dim() == 3:
+        frames = frames[None]
+    if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+        raise LwbError("frames must be uint8 [n,H,W,3] or [H,W,3], got %s %s"
+                       % (str(frames.dtype).replace("torch.", ""), list(frames.shape)))
+    n, h, w, _ = frames.shape
+    dev = frames.device
+    img = torch.empty((n, 3, size, size), dtype=torch.float32, device=dev) if want_img else None
+    hmr = torch.empty((n, 3, hmr_size, hmr_size), dtype=torch.float32, device=dev) if want_hmr else None
+    u8 = torch.empty((n, size, size, 3), dtype=torch.uint8, device=dev) if want_u8 else None
+    _count(1)
+    check(lib().lwb_frames_in(ptr(frames), n, h, w, int(bool(bgr)), size, ptr(img), hmr_size, ptr(hmr), ptr(u8), stream()),
+          "lwb_frames_in")
+    return img, hmr, u8
+
+
 def conv2d_direct_nchw(x, w, bias=None, stride=1, pad=0, dil=1):
     _chk_cuda(x, w, bias)
     n, cin, h, wd = x.shape

@@ -56,8 +56,8 @@ class Swapper(Imitator):
     # ---- personalize: returns the info instead of storing it (models/swapper.py:99-165) --------
     @_on_device
     @torch.no_grad()
-    def personalize(self, src_path, src_smpl=None, output_path='', visualizer=None, src_img=None):
-        return self._personalize(src_path, src_smpl, output_path, None, src_img)
+    def personalize(self, src_path, src_smpl=None, output_path='', visualizer=None, src_img=None, src_frame=None):
+        return self._personalize(src_path, src_smpl, output_path, None, src_img, src_frame)
 
     def _extend_src_info(self, src_info):
         src_info['part'], _ = self.render.encode_fim(src_info['cam'], src_info['verts'], fim=src_info['fim'],
@@ -75,9 +75,11 @@ class Swapper(Imitator):
 
     @_on_device
     @torch.no_grad()
-    def swap_setup(self, src_path, tgt_path, src_smpl=None, tgt_smpl=None, output_dir='', src_img=None, tgt_img=None):
-        self.src_info = self.personalize(src_path, src_smpl, src_img=src_img)
-        self.tsf_info = self.personalize(tgt_path, tgt_smpl, src_img=tgt_img)
+    def swap_setup(self, src_path, tgt_path, src_smpl=None, tgt_smpl=None, output_dir='', src_img=None, tgt_img=None,
+                   src_frame=None, tgt_frame=None):
+        """``src_frame`` / ``tgt_frame`` (extension): uint8 [H,W,3] BGR frames in place of the files (Imitator.personalize)."""
+        self.src_info = self.personalize(src_path, src_smpl, src_img=src_img, src_frame=src_frame)
+        self.tsf_info = self.personalize(tgt_path, tgt_smpl, src_img=tgt_img, src_frame=tgt_frame)
 
     @_on_device
     @torch.no_grad()

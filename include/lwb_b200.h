@@ -246,6 +246,15 @@ int lwb_heads_composite(const float* raw, int n, int h, int w, int c_stride, int
  * (e.g. after Imitator.warp_front, models/imitator.py:338-342). */
 int lwb_frames_out(const float* frames, int n, int h, int w, float* hwc, uint8_t* u8_bgr, lwb_stream_t stream);
 
+/* Input path: n uint8 frames [n,h,w,3] (bgr = 1: B,G,R as cv2.imread returns them; 0: R,G,B), all one size, resized the
+ * way cv2.resize(frame, (s, s)) resizes uint8 with INTER_LINEAR -- the same bytes -- and written in one launch to any of
+ *   img    [n,3,size,size]         fp32 RGB, x / 255.0 * 2 - 1.0 in fp32 (utils/cv_utils.py:10-47 + models/imitator.py:89),
+ *   hmr    [n,3,hmr_size,hmr_size] fp32 RGB, the same formula, resized from the frame itself (the HMR input),
+ *   u8_bgr [n,size,size,3]         uint8 BGR, what cv_utils.save_cv2_img(frame, image_size=size) hands to cv2.imwrite.
+ * A null output is skipped; at least one must be given. */
+int lwb_frames_in(const uint8_t* frames, int n, int h, int w, int bgr, int size, float* img, int hmr_size,
+                  float* hmr, uint8_t* u8_bgr, lwb_stream_t stream);
+
 /* Direct (CUDA-core) convolution, NCHW fp32, arbitrary kernel / stride / dilation, optional bias:
  * the once-per-source inpaintor layers (networks/inpaintor.py:12-47) and odd shapes. */
 int lwb_conv2d_direct_nchw(const float* x, const float* w, const float* bias,
