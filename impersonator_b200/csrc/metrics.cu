@@ -219,12 +219,21 @@ extern "C" int lwb_ssim_psnr(const float* pred, const float* ref, int n, int h, 
                              double* ssim_out, double* psnr_out, lwb_stream_t stream)
 {
     LWB_CHECK_ARG(pred && ref && workspace && ssim_out && psnr_out, "null pointer");
-    LWB_CHECK_ARG(n > 0 && n <= 65535 / 3 && h >= 7 && w >= 7, "bad sizes (the 7x7 window needs h, w >= 7)");
-    dim3 grid(lwb::ceil_div(w, ST_W), lwb::ceil_div(h, ST_H), n * 3);
-    LWB_CHECK_ARG(grid.y <= 65535, "image too tall");
-    k_ssim_tiles<<<grid, S_THREADS, 0, (cudaStream_t)stream>>>(pred, ref, h, w, from01 ? 1 : 0, (double3*)workspace);
-    LWB_LAUNCH_OK();
-    k_ssim_finish<<<n, S_THREADS, 0, (cudaStream_t)stream>>>((const double3*)workspace, (int)(grid.x * grid.y), h, w,
+    LWB_CHECK_ARG(n > 0 && h >= 7 && w >= 7, "bad sizes (the 7x7 window needs h, w >= 7)");
+    const int gx = lwb::ceil_div(w, ST_W), gy = lwb::ceil_div(h, ST_H);
+    LWB_CHECK_ARG(gy <= 65535, "image too tall");
+    // grid.z holds 3 planes per frame and stops at 65535: the tiles of larger batches run in chunks of frames, each
+    // writing its own part of the workspace; one k_ssim_finish then reduces every frame.
+    constexpr int max_frames = 65535 / 3;
+    const size_t plane = (size_t)h * w, tiles = (size_t)gx * gy;
+    for (int i0 = 0; i0 < n; i0 += max_frames) {
+        const int m = n - i0 < max_frames ? n - i0 : max_frames;
+        k_ssim_tiles<<<dim3(gx, gy, m * 3), S_THREADS, 0, (cudaStream_t)stream>>>(
+            pred + (size_t)i0 * 3 * plane, ref + (size_t)i0 * 3 * plane, h, w, from01 ? 1 : 0,
+            (double3*)workspace + (size_t)i0 * 3 * tiles);
+        LWB_LAUNCH_OK();
+    }
+    k_ssim_finish<<<n, S_THREADS, 0, (cudaStream_t)stream>>>((const double3*)workspace, (int)tiles, h, w,
                                                             ssim_out, psnr_out);
     LWB_LAUNCH_OK();
     return LWB_OK;

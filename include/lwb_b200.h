@@ -380,7 +380,8 @@ int lwb_det_person_mask(const float* boxes, const int* labels, const int* count,
  *   ssim_psnr     per frame: skimage 0.16.2 structural_similarity(pred, ref, multichannel=True) on the HWC image (7x7
  *                 uniform window, sample covariance, K1 0.01, K2 0.03, data_range 2, map cropped by 3, mean per channel
  *                 then over channels) and peak_signal_noise_ratio(image_true=ref, image_test=pred) (data_range 1 when
- *                 min(ref) >= 0, else 2; +inf for identical frames), both fp64 [n].  h, w >= 7.  workspace:
+ *                 min(ref) >= 0, else 2; +inf for identical frames), both fp64 [n].  h, w >= 7; n has no upper
+ *                 limit (batches of more than 21845 frames run their tiles in several launches).  workspace:
  *                 lwb_ssim_psnr_workspace_bytes(n, h, w) bytes.  Fixed-order reductions: results repeat bit for bit.
  *   lpips_input   PNetLin's scaling layer (x - shift) / scale of pred and ref stacked as one batch: out [2n,3,h,w]
  *                 (pred first), the input of the AlexNet features (conv1 via lwb_conv2d_direct_relu_nhwc, the pools via
