@@ -59,26 +59,19 @@ def morph(src_bg_mask, ks, mode='erode'):
     return (pooled.round() >= 1).float()
 
 
-def _read_image(path, image_size):
-    """cv_utils.read_cv2_img + transform_img (utils/cv_utils.py:10-47) -> RGB float32 CHW in [0,1], original."""
+def _read_image(path):
+    """cv_utils.read_cv2_img (utils/cv_utils.py:10-20) -> the decoded RGB uint8 [H,W,3] image, which then takes the
+    frame route (kernels.frames_in, bgr=False).  Unlike the reference, which scales a 16-bit PNG to values up to 513,
+    anything but an 8-bit 3-channel image raises LwbError."""
     import cv2
     img = cv2.imread(path, -1)
     if img is None:
         raise IOError("cannot read %s" % path)
     img = cv2.cvtColor(img, cv2.COLOR_BGR2RGB)
-    x = cv2.resize(img, (image_size, image_size)).astype(np.float32) / 255.0
-    return x.transpose((2, 0, 1)), img
-
-
-def _save_image(img, path, image_size=None, normalize=False):
-    """cv_utils.save_cv2_img (utils/cv_utils.py:23-36)."""
-    import cv2
-    img = cv2.cvtColor(img, cv2.COLOR_RGB2BGR)
-    if image_size is not None:
-        img = cv2.resize(img, (image_size, image_size))
-    if normalize:
-        img = ((img + 1) / 2.0 * 255).astype(np.uint8)
-    cv2.imwrite(path, img)
+    if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
+        raise LwbError("%s decodes to %s %s: only 8-bit images with 3 colour channels are read"
+                       % (path, img.dtype, list(img.shape)))
+    return img
 
 
 def _frame_stack(frames):
@@ -224,8 +217,9 @@ class Imitator(object):
     @torch.no_grad()
     def personalize(self, src_path, src_smpl=None, output_path='', visualizer=None, src_img=None, src_frame=None):
         """models/imitator.py:82-145.  ``src_frame`` (extension): one uint8 frame [H,W,3], B,G,R as cv2.imread returns it,
-        on the host or the device, in place of the file at ``src_path`` (which may then be '').  It is resized on the
-        device exactly as the file would be (kernels.frames_in), and ``src_info['image']`` keeps it as given."""
+        on the host or the device, in place of the file at ``src_path`` (which may then be '').  A file is decoded and
+        takes the same route: resized on the device byte for byte as OpenCV resizes (kernels.frames_in).
+        ``src_info['image']`` is the frame as given, or the file's RGB image."""
         self.src_info = self._personalize(src_path, src_smpl, output_path, visualizer, src_img, src_frame)
         self.__dict__['_graphs'] = {}                    # captured chunk graphs hold the previous source's buffers
 
@@ -239,26 +233,18 @@ class Imitator(object):
 
     def _personalize(self, src_path, src_smpl=None, output_path='', visualizer=None, src_img=None, src_frame=None):
         """The body shared by models/imitator.py:82-145, models/viewer.py:83-143 and models/swapper.py:99-165 -> src_info."""
-        size = self._opt.image_size
+        if src_frame is not None and src_img is not None:
+            raise LwbError("give the source as src_img or as src_frame, not both")
         img_hmr = gt_u8 = None
-        if src_frame is not None:
-            if src_img is not None:
-                raise LwbError("give the source as src_img or as src_frame, not both")
-            img, img_hmr, gt_u8 = K.frames_in(src_frame, size, want_hmr=src_smpl is None and self.hmr is not None,
-                                              want_u8=bool(output_path))
-            ori_img = src_frame
-        elif src_img is None:
-            img, ori_img = _read_image(src_path, size)
-            img = torch.tensor(img * 2 - 1.0, dtype=torch.float32, device=self.device)[None, ...]
+        if src_img is None:
+            ori_img = src_frame if src_frame is not None else _read_image(src_path)
+            img, img_hmr, gt_u8 = K.frames_in(ori_img, self._opt.image_size, bgr=src_frame is not None,
+                                              want_hmr=src_smpl is None and self.hmr is not None, want_u8=bool(output_path))
         else:
             img, ori_img = src_img.to(self.device).float(), None
         if src_smpl is None:
-            if self.hmr is None or ori_img is None:
-                raise LwbError("src_smpl required when no HMR network is injected")
             if img_hmr is None:
-                import cv2
-                img_hmr = cv2.resize(ori_img, (224, 224)).astype(np.float32).transpose((2, 0, 1)) / 255.0 * 2 - 1.0
-                img_hmr = torch.tensor(img_hmr, dtype=torch.float32, device=self.device)[None, ...]
+                raise LwbError("src_smpl required when no HMR network is injected")
             src_smpl = self.hmr(img_hmr)
         else:
             src_smpl = torch.as_tensor(src_smpl, dtype=torch.float32, device=self.device).reshape(1, -1)
@@ -296,11 +282,9 @@ class Imitator(object):
         if visualizer is not None:
             visualizer.vis_named_img('src', img)
             visualizer.vis_named_img('bg', src_info['bg'])
-        if output_path and gt_u8 is not None:
+        if gt_u8 is not None:
             import cv2
             cv2.imwrite(output_path, gt_u8[0].cpu().numpy())
-        elif output_path and ori_img is not None:
-            _save_image(ori_img, output_path, image_size=size)
         return src_info
 
     # ---- per-frame geometry (models/imitator.py:216-268) --------------------------------------
@@ -387,17 +371,15 @@ class Imitator(object):
         stage = lambda t: t.clone() if t is not None else None
         return dict(tsf_info=res['tsf_info'], preds=res['preds'], hwc=stage(res['hwc']), u8=stage(res['u8']), flag=stage(res['flag']))
 
+    @_on_device
     @torch.no_grad()
     def transfer_params(self, tgt_path, tgt_smpl=None, cam_strategy='smooth', t=0):
-        ori_img = None
-        if tgt_path:
-            _, ori_img = _read_image(tgt_path, self._opt.image_size)
+        ori_img = _read_image(tgt_path) if tgt_path else None
         if tgt_smpl is None:
             if self.hmr is None or ori_img is None:
                 raise LwbError("tgt_smpl required when no HMR network is injected")
-            import cv2
-            img_hmr = cv2.resize(ori_img, (224, 224)).astype(np.float32).transpose((2, 0, 1)) / 255.0 * 2 - 1.0
-            tgt_smpl = self.hmr(torch.tensor(img_hmr, dtype=torch.float32, device=self.device)[None, ...])
+            _, img_hmr, _ = K.frames_in(ori_img, self._opt.image_size, bgr=False, want_img=False)
+            tgt_smpl = self.hmr(img_hmr)
         tsf_inputs = self.transfer_params_by_smpl(tgt_smpl=tgt_smpl, cam_strategy=cam_strategy, t=t)
         self.tsf_info['image'] = ori_img
         return tsf_inputs
@@ -457,12 +439,15 @@ class Imitator(object):
         LPIPS when an ``lpips`` = metrics.LPIPS is given), and the call returns (outputs, scores) with scores a dict of
         per-frame float64 numpy arrays.
 
+        The target images are read only when the HMR input (``tgt_smpls=None``) or the gt_ images (``output_dir``) need
+        them; with given SMPL vectors and neither, only the last file is read, for ``tsf_info['image']``.  Each chunk of
+        them is resized on the device (kernels.frames_in: one launch, or one per image when decoded files differ in
+        size), byte for byte as OpenCV resizes; a host chunk is uploaded on the copy stream one chunk ahead.
+
         ``tgt_frames`` (extension): the target frames themselves instead of files -- uint8 [N,H,W,3], B,G,R as cv2.imread
         returns them, a numpy array or a tensor on the host or the device, or a sequence of [H,W,3] frames of one size.
-        ``tgt_paths`` must then be empty or all ''.  Each chunk's frames are resized on the device in one launch
-        (kernels.frames_in) into the HMR input and, with ``output_dir``, the gt_ images, byte for byte what the file route
-        computes; a host source is uploaded on the copy stream one chunk ahead.  ``tsf_info['image']`` is the last frame
-        as given; the files are named like inference_by_smpls names them (gt_%.8d.jpg beside pred_%.8d.jpg)."""
+        ``tgt_paths`` must then be empty or all ''.  ``tsf_info['image']`` is the last frame as given; the files are named
+        like inference_by_smpls names them (gt_%.8d.jpg beside pred_%.8d.jpg)."""
         if tgt_frames is not None:
             tgt_frames = _frame_stack(tgt_frames)
             if tgt_paths and (any(tgt_paths) or len(tgt_paths) != len(tgt_frames)):
@@ -474,161 +459,151 @@ class Imitator(object):
             from . import metrics as _metrics
             if len(score_against) != length:
                 raise LwbError("score_against holds %d frames for %d targets" % (len(score_against), length))
-            scores = []
-        outputs = []
-        last_image = [None]
-        originals = {}                                           # frame index -> original RGB image (for the gt_ files)
-
-        frame_u8 = {}                                            # chunk start -> its gt_ images, BGR uint8 on the device
-
-        def chunk_smpls(a, b):
-            """SMPL vectors of frames a..b-1: given, or estimated from the target images by HMR -- one encoder batch per
-            chunk instead of one launch sequence per frame (models/imitator.py:271-275)."""
-            if tgt_frames is not None:
-                want_hmr = tgt_smpls is None
-                if want_hmr and (self.hmr is None or not callable(self.hmr)):
-                    raise LwbError("tgt_smpls required when no HMR network is available")
-                last_image[0] = tgt_frames[b - 1]
-                if want_hmr or output_dir:
-                    _, hmr_in, gt = K.frames_in(chunk_frames(a, b), self._opt.image_size, want_img=False,
-                                                want_hmr=want_hmr, want_u8=bool(output_dir))
-                    if gt is not None:
-                        frame_u8[a] = gt
-                if not want_hmr:
-                    return torch.as_tensor(np.stack([np.asarray(s, dtype=np.float32).reshape(-1) for s in tgt_smpls[a:b]]))
-                return self.hmr(hmr_in)
-            if tgt_smpls is not None:
-                return torch.as_tensor(np.stack([np.asarray(s, dtype=np.float32).reshape(-1) for s in tgt_smpls[a:b]]))
-            if self.hmr is None or not callable(self.hmr):
-                raise LwbError("tgt_smpls required when no HMR network is available")
-            import cv2
-            batch = []
-            for k, path in enumerate(tgt_paths[a:b]):
-                _, ori = _read_image(path, self._opt.image_size)
-                batch.append(cv2.resize(ori, (224, 224)).astype(np.float32).transpose((2, 0, 1)) / 255.0 * 2 - 1.0)
-                last_image[0] = ori
-                if output_dir:
-                    originals[a + k] = ori
-            return self.hmr(torch.from_numpy(np.stack(batch)).to(self.device))
+        want_hmr = tgt_smpls is None                             # one HMR batch per chunk (models/imitator.py:271-275)
+        if want_hmr and length and (self.hmr is None or not callable(self.hmr)):
+            raise LwbError("tgt_smpls required when no HMR network is available")
+        want_gt = bool(output_dir) and (tgt_frames is not None or any(tgt_paths))
         # Chunks are pipelined: the D2H of chunk i runs on a copy stream while chunk i+1 computes; the host only
         # waits for a chunk's copy when it has already queued the next chunk (and once at the end).
         main = torch.cuda.current_stream(self.device)
         if getattr(self, '_copy_stream', None) is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
-        pending = []
-        range_bits = [0]
-        uploads = {}                                             # chunk start -> (frames on the device, copy finished)
-        host_frames = tgt_frames is not None and not (torch.is_tensor(tgt_frames) and tgt_frames.is_cuda)
+        chunks = self._chunks(length)
 
-        def upload(a, b):
-            """H2D of a host chunk on the copy stream (two staging slots: one chunk in flight while the next is filled)."""
+        def upload(i):
+            """Target images of chunk i -- the given frames, or the decoded files: one [n,H,W,3] array, or one per image
+            when they differ in size -- H2D on the copy stream (two staging slots: one chunk in flight while the next is
+            filled)."""
+            a, b = chunks[i]
+            if tgt_frames is not None:
+                host = tgt_frames[a:b]
+                parts = [host]
+            else:
+                host = [_read_image(p) for p in tgt_paths[a:b]]
+                parts = [np.stack(host)] if len({x.shape for x in host}) == 1 else host
             with torch.cuda.stream(self._copy_stream):
-                dev = K.upload_u8(tgt_frames[a:b], self.device, slot=chunks.index((a, b)) % 2)
+                dev = [K.upload_u8(x, self.device, slot=i % 2) for x in parts]
                 done = torch.cuda.Event()
                 done.record(self._copy_stream)
-            dev.record_stream(main)
-            uploads[a] = (dev, done)
+            for d in dev:
+                d.record_stream(main)
+            return host, dev, done
 
-        def chunk_frames(a, b):
-            if not host_frames:
-                return tgt_frames[a:b]
-            if a not in uploads:
-                upload(a, b)
-            dev, done = uploads.pop(a)
-            main.wait_event(done)
-            nxt = [(c, d) for (c, d) in chunks if c == b]
-            if nxt:
-                upload(*nxt[0])                                  # overlaps this chunk's generator pass
-            return dev
+        def chunk_images():
+            """(target images on the host or None, on the device) of each chunk in turn."""
+            if torch.is_tensor(tgt_frames) and tgt_frames.is_cuda:
+                for a, b in chunks:
+                    yield None, [tgt_frames[a:b]]
+                return
+            nxt = upload(0)
+            for i in range(len(chunks)):
+                host, dev, done = nxt
+                main.wait_event(done)
+                if i + 1 < len(chunks):
+                    nxt = upload(i + 1)                          # overlaps this chunk's generator pass
+                yield host, dev
 
-        def drain(keep):
+        def drain(pending, keep, outputs):
+            """Waits for the D2H of all but ``keep`` pending chunks, hands out their frames -> their operand-range bits."""
+            bits = 0
             while len(pending) > keep:
                 a0, b0, h_f, h_u8, h_gt, h_flag, done = pending.pop(0)
                 done.synchronize()
                 if h_flag is not None:
-                    range_bits[0] |= int(h_flag[0])
+                    bits |= int(h_flag[0])
                 host = h_u8 if as_uint8 else h_f
                 for j in range(b0 - a0):
                     outputs.append(host[j])
                     if output_dir:
-                        self._maybe_save(h_u8[j], tgt_paths[a0 + j], output_dir, a0 + j, is_bgr_u8=True,
-                                         original=originals.pop(a0 + j, None),
-                                         gt_u8=h_gt[j] if h_gt is not None else None)
+                        self._maybe_save(h_u8[j], tgt_paths[a0 + j], output_dir, a0 + j,
+                                         h_gt[j] if h_gt is not None else None)
+            return bits
 
-        chunks = self._chunks(length)
-        for (a, b) in chunks:
-            smpls = torch.as_tensor(chunk_smpls(a, b), dtype=torch.float32).to(self.device, non_blocking=True)
-            if smpls.dim() == 1:
-                smpls = smpls[None, ...]
-            if a == 0 and cam_strategy == 'smooth':
-                self._set_first_cam(smpls[0:1, 0:3])
-            want_u8 = bool(as_uint8 or output_dir)
-            res = self._chunk_step(smpls, cam_strategy, not as_uint8, want_u8)
-            out_hwc, out_u8, flag = res['hwc'], res['u8'], res['flag']
-            if score_against is not None:
-                gt = _metrics._frames(score_against[a:b], self.device)
-                scores.append(_metrics.score_frames(res['preds'], gt, from01=False, lpips=lpips))
-            if visualizer is not None:
-                visualizer.vis_named_img('pred_' + cam_strategy, res['preds'])
-            ready = torch.cuda.Event()
-            ready.record(main)
-            with torch.cuda.stream(self._copy_stream):
-                self._copy_stream.wait_event(ready)
-                h_f = self._to_host(out_hwc, sync=False) if not as_uint8 else None
-                h_u8 = self._to_host(out_u8, sync=False) if want_u8 else None
-                h_flag = self._to_host(flag, sync=False) if flag is not None else None
-                gt = frame_u8.pop(a, None)
-                h_gt = self._to_host(gt, sync=False) if gt is not None else None
-                for t in (out_hwc, out_u8, flag, gt):
-                    if t is not None:
-                        t.record_stream(self._copy_stream)
-                done = torch.cuda.Event()
-                done.record(self._copy_stream)
-            pending.append((a, b, h_f, h_u8, h_gt, h_flag, done))
-            drain(keep=1)
-        drain(keep=0)
+        def run():
+            """One pass over the chunks -> (outputs, per-chunk scores, operand-range bits)."""
+            outputs, scores, pending, bits = [], [], [], 0
+            last = tgt_frames[-1] if tgt_frames is not None and length else None
+            images = chunk_images() if want_hmr or want_gt else None
+            for (a, b) in chunks:
+                hmr_in = gt = None
+                if images is not None:
+                    host, dev = next(images)
+                    outs = [K.frames_in(d, self._opt.image_size, bgr=tgt_frames is not None, want_img=False,
+                                        want_hmr=want_hmr, want_u8=want_gt)[1:] for d in dev]
+                    hmr_in, gt = outs[0] if len(outs) == 1 else [None if o[0] is None else torch.cat(o) for o in zip(*outs)]
+                    if tgt_frames is None:
+                        last = host[-1]
+                if want_hmr:
+                    smpls = self.hmr(hmr_in)
+                else:
+                    smpls = np.stack([np.asarray(s, dtype=np.float32).reshape(-1) for s in tgt_smpls[a:b]])
+                smpls = torch.as_tensor(smpls, dtype=torch.float32).to(self.device, non_blocking=True)
+                if smpls.dim() == 1:
+                    smpls = smpls[None, ...]
+                if a == 0 and cam_strategy == 'smooth':
+                    self._set_first_cam(smpls[0:1, 0:3])
+                want_u8 = bool(as_uint8 or output_dir)
+                res = self._chunk_step(smpls, cam_strategy, not as_uint8, want_u8)
+                out_hwc, out_u8, flag = res['hwc'], res['u8'], res['flag']
+                if score_against is not None:
+                    scores.append(_metrics.score_frames(res['preds'], _metrics._frames(score_against[a:b], self.device),
+                                                        from01=False, lpips=lpips))
+                if visualizer is not None:
+                    visualizer.vis_named_img('pred_' + cam_strategy, res['preds'])
+                ready = torch.cuda.Event()
+                ready.record(main)
+                with torch.cuda.stream(self._copy_stream):
+                    self._copy_stream.wait_event(ready)
+                    h_f = self._to_host(out_hwc, sync=False) if not as_uint8 else None
+                    h_u8 = self._to_host(out_u8, sync=False) if want_u8 else None
+                    h_flag = self._to_host(flag, sync=False) if flag is not None else None
+                    h_gt = self._to_host(gt, sync=False) if gt is not None else None
+                    for t in (out_hwc, out_u8, flag, gt):
+                        if t is not None:
+                            t.record_stream(self._copy_stream)
+                    done = torch.cuda.Event()
+                    done.record(self._copy_stream)
+                pending.append((a, b, h_f, h_u8, h_gt, h_flag, done))
+                bits |= drain(pending, 1, outputs)
+            bits |= drain(pending, 0, outputs)
+            self._last_frame_info()
+            if last is None and length and tgt_paths[-1]:
+                # driven by given SMPL vectors AND frame files (evaluate.py:62): transfer_params still reads every frame file
+                # (models/imitator.py:270) and leaves the last one in tsf_info['image']; only that one is read here
+                last = _read_image(tgt_paths[-1])
+            if last is not None:
+                self.tsf_info['image'] = last
+            return outputs, scores, bits
 
-        def result():
-            if score_against is None:
-                return outputs
-            keys = scores[0].keys() if scores else ("ssim", "psnr")
-            return outputs, {k: torch.cat([s[k].double() for s in scores]).cpu().numpy() if scores else np.zeros(0)
-                             for k in keys}
-        self._last_frame_info()
-        if last_image[0] is None and length and tgt_paths[-1] and self.tsf_info:
-            # driven by given SMPL vectors AND frame files (evaluate.py:62): transfer_params still reads every frame file
-            # (models/imitator.py:270) and leaves the last one in tsf_info['image']; only that one is read here
-            _, last_image[0] = _read_image(tgt_paths[-1], self._opt.image_size)
-        if last_image[0] is not None:
-            self.tsf_info['image'] = last_image[0]
-        if range_bits[0] and not getattr(self, '_range_retry', False):
+        outputs, scores, bits = run()
+        if bits:
             # Never silently: activations left the range in which the default fp16f8 operand split keeps its precision
             # (RANGE_F8: |x| >= 1024, the e4m3 correction terms clip; RANGE_HEADS: output-head pre-activations of +-8 and
             # more, where its ~1e-4 relative precision may exceed 1e-3 on pixels).  Pin the generator to fp16x3 (fp16
-            # corrections, range 6e4) and redo the call -- LWB_AUTO_PRECISION=0 only warns; beyond the fp16 range
+            # corrections, range 6e4) and redo the pass -- LWB_AUTO_PRECISION=0 only warns; beyond the fp16 range
             # (RANGE_FP16) nothing in this engine can represent the activations.
             import warnings
-            if range_bits[0] & RANGE_FP16:
+            if bits & RANGE_FP16:
                 raise LwbError("generator activations exceed the fp16 range (|x| >= 6e4 or non-finite): the conv engine's "
                                "fp16 operands cannot represent them")
-            what = ("activations beyond the fp16f8 correction range (|x| >= 1024)" if range_bits[0] & RANGE_F8 else
+            what = ("activations beyond the fp16f8 correction range (|x| >= 1024)" if bits & RANGE_F8 else
                     "output-head pre-activations beyond +-8 (fp16f8's ~1e-4 relative precision may exceed 1e-3 on pixels)")
             if os.environ.get("LWB_AUTO_PRECISION", "1") == "0" or getattr(self.generator, '_lwb_precision', None) == "fp16x3" \
                     or os.environ.get("LWB_PRECISION", "fp16f8") != "fp16f8":
                 warnings.warn("lwb_b200: %s (precision mode kept)" % what)
-                return result()
-            warnings.warn("lwb_b200: %s; switching this generator to LWB_PRECISION=fp16x3 and recomputing the sequence" % what)
-            self.generator.set_precision("fp16x3")
-            self._range_retry = True
-            try:
+            else:
+                warnings.warn("lwb_b200: %s; switching this generator to LWB_PRECISION=fp16x3 and recomputing the sequence"
+                              % what)
+                self.generator.set_precision("fp16x3")
                 enc_in = self.src_info.get('src_inputs')
                 if enc_in is not None:
                     self.src_info['feats'] = self.generator.encode_src(enc_in)
-                return self.inference(tgt_paths, tgt_smpls, cam_strategy, output_dir, visualizer, verbose, as_uint8,
-                                      score_against, lpips, tgt_frames)
-            finally:
-                self._range_retry = False
-        return result()
+                outputs, scores, _ = run()                       # the fp16x3 pass is final: its range bits are not checked
+        if score_against is None:
+            return outputs
+        keys = scores[0].keys() if scores else ("ssim", "psnr")
+        return outputs, {k: torch.cat([s[k].double() for s in scores]).cpu().numpy() if scores else np.zeros(0)
+                         for k in keys}
 
     @torch.no_grad()
     def inference_by_smpls(self, tgt_smpls, cam_strategy='smooth', output_dir='', visualizer=None, as_uint8=False):
@@ -654,26 +629,15 @@ class Imitator(object):
                 info[k] = v[-1:].clone()                 # own storage: the chunk buffers may belong to a replayed graph
         self.tsf_info = info
 
-    def _maybe_save(self, pred, tgt_path, output_dir, t, is_bgr_u8=False, original=None, gt_u8=None):
-        """pred_<file> (+ gt_<file> = the driving frame resized, models/imitator.py:182-187); inference_by_smpls names
-        its frames pred_%.8d.jpg (:212).  ``gt_u8``: the driving frame already resized (BGR uint8), written as
-        gt_<file>, or gt_%.8d.jpg where there is no file name."""
-        if not output_dir:
-            return
-        name = os.path.split(tgt_path)[-1] if tgt_path else 'pred_%.8d.jpg' % t
-        path = os.path.join(output_dir, 'pred_' + name if tgt_path else name)
+    @staticmethod
+    def _maybe_save(pred_u8, tgt_path, output_dir, t, gt_u8=None):
+        """pred_<file> and, when given, gt_<file> = the driving frame resized (models/imitator.py:182-187), from BGR uint8
+        images; without a file name pred_%.8d.jpg (inference_by_smpls, :212) and gt_%.8d.jpg."""
+        import cv2
+        name = os.path.split(tgt_path)[-1]
         if gt_u8 is not None:
-            import cv2
-            cv2.imwrite(os.path.join(output_dir, 'gt_' + name if tgt_path else 'gt_%.8d.jpg' % t), gt_u8)
-        elif tgt_path:
-            if original is None:
-                _, original = _read_image(tgt_path, self._opt.image_size)
-            _save_image(original, os.path.join(output_dir, 'gt_' + name), image_size=self._opt.image_size)
-        if is_bgr_u8:
-            import cv2
-            cv2.imwrite(path, pred)                      # already what save_cv2_img(normalize=True) would write
-        else:
-            _save_image(pred, path, normalize=True)
+            cv2.imwrite(os.path.join(output_dir, 'gt_' + name if name else 'gt_%.8d.jpg' % t), gt_u8)
+        cv2.imwrite(os.path.join(output_dir, 'pred_' + name if name else 'pred_%.8d.jpg' % t), pred_u8)
 
     def post_personalize(self, *a, **k):
         raise LwbError("post_personalize (fine-tuning) needs the backward pass: outside the inference hot path")

@@ -81,8 +81,9 @@ def frames(n, h, w, seed):
 
 
 def cv2_route(frame, size, bgr=True, hmr_size=HMR_SIZE):
-    """What the file route of Imitator computes from one frame (imitator.py _read_image, the HMR resize, _save_image):
-    -> (img [3,S,S] fp32, hmr [3,224,224] fp32, gt_ image [S,S,3] uint8 BGR)."""
+    """What the reference computes from one decoded frame with cv2 on the host (utils/cv_utils.py read_cv2_img,
+    transform_img and save_cv2_img, the HMR resize of models/imitator.py:271-275), the result lwb_frames_in must
+    reproduce: -> (img [3,S,S] fp32, hmr [3,224,224] fp32, gt_ image [S,S,3] uint8 BGR)."""
     import cv2
     rgb = cv2.cvtColor(frame, cv2.COLOR_BGR2RGB) if bgr else frame
     img = (cv2.resize(rgb, (size, size)).astype(np.float32) / 255.0).transpose((2, 0, 1)) * 2 - 1.0

@@ -1112,6 +1112,7 @@ COVERED_ELSEWHERE = {
     "bn_act_segment": "test_inception_gpu.py::test_bn_act_segment_matches_float64",
     "inception_input": "test_inception_gpu.py::test_input_matches_interpolate",
     "_correspond": "test_raster_gpu.py::test_correspond_matches_oracle",
+    "frames_in": "test_frames_in_gpu.py::test_frames_in_matches_cv2_route",
 }
 
 

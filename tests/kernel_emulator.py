@@ -6,10 +6,12 @@ wrong.  ``install(monkeypatch)`` replaces every kernel front-end the streams cal
 SAME contract (include/lwb_b200.h), so the CPU suite can run the whole host logic against the oracles.  The emulation
 works on the fp16 hi/lo operand pairs (run it with LWB_PRECISION=fp16x3); it is never used by the product.
 """
+import numpy as np
 import torch
 import torch.nn.functional as F
 
 from conv_emulation import act_pair_blocks, fp16_pair, range_bits
+from frames_in_cases import cv2_route
 from impersonator_b200 import kernels as K
 from impersonator_b200.binding import RANGE_HEADS
 
@@ -420,11 +422,21 @@ def inception_input(x, out=None):
     return out
 
 
+def frames_in(frames, size, hmr_size=224, bgr=True, want_img=True, want_hmr=True, want_u8=False):
+    """lwb_frames_in's contract through cv2 itself (frames_in_cases.cv2_route), frame by frame, into host tensors."""
+    a = frames.cpu().numpy() if torch.is_tensor(frames) else np.asarray(frames)
+    routes = [cv2_route(f, size, bgr=bgr, hmr_size=hmr_size) for f in (a[None] if a.ndim == 3 else a)]
+    return tuple(torch.from_numpy(np.stack([r[k] for r in routes])) if want else None
+                 for k, want in enumerate((want_img, want_hmr, want_u8)))
+
+
 def install_tasks(monkeypatch):
-    """install() + the correspondence / warp front-ends and the renderer's CUDA-only guard: enough to run the task classes'
-    personalize / view / swap on CPU (Imitator.inference itself drives CUDA streams and stays GPU-only)."""
+    """install() + the input-path, correspondence and warp front-ends and the renderer's CUDA-only guard: enough to run
+    the task classes' personalize / view / swap on CPU (Imitator.inference itself drives CUDA streams and stays
+    GPU-only)."""
     from impersonator_b200 import nmr
     install(monkeypatch)
+    monkeypatch.setattr(K, "frames_in", frames_in)
     monkeypatch.setattr(K, "correspond", correspond)
     monkeypatch.setattr(K, "warp_nchw", warp_nchw)
 

@@ -90,3 +90,26 @@ def test_frame_stack_refuses_mixed_sizes_and_dtypes():
     with pytest.raises(_lib.LwbError, match="uint8"):
         _frame_stack(np.zeros((2, 4, 4), np.uint8))
     assert _frame_stack([np.ones((4, 5, 3), np.uint8)] * 3).shape == (3, 4, 5, 3)
+
+
+def test_a_16_bit_png_is_refused_naming_the_file(tmp_path, monkeypatch):
+    """A 16-bit PNG decodes to uint16, which the reference's float conversion would scale to values up to 513: the
+    Imitator raises before anything is computed, naming the file."""
+    import kernel_emulator
+    import tasks_common as C
+    from impersonator_b200 import synthetic as S
+    from impersonator_b200.generator import ImpersonatorGenerator
+    from impersonator_b200.imitator import Imitator
+    from impersonator_b200.nmr import SMPLRenderer
+    kernel_emulator.install_tasks(monkeypatch)
+    v, f = S.uv_sphere()
+    path = str(tmp_path / "deep.png")
+    assert cv2.imwrite(path, F.frames(1, 40, 30, seed=5)[0].astype(np.uint16) * 257)
+    assert cv2.imread(path, -1).dtype == np.uint16
+    render = SMPLRenderer(image_size=C.SIZE, faces=f.numpy(), map_fn=S.synthetic_tables()["map_fn"])
+    im = Imitator(C.Opt(), generator=ImpersonatorGenerator(bg_dim=4, src_dim=6, tsf_dim=6, repeat_num=6),
+                  hmr=S.QuarterTurnBodyModel(v), render=render, device="cpu")
+    with pytest.raises(_lib.LwbError, match="deep.png decodes to uint16"):
+        im.personalize(path, src_smpl=np.zeros(85, np.float32))
+    with pytest.raises(_lib.LwbError, match="deep.png decodes to uint16"):
+        im.transfer_params(path, tgt_smpl=np.zeros(85, np.float32))

@@ -181,6 +181,50 @@ def test_inference_frames_with_given_smpls_and_argument_conflicts(cuda, world):
         im.inference([], tgt_frames=[world["frames"][0], world["frames"][0][:100]])
 
 
+def test_inference_over_files_of_two_sizes(cuda, world, tmp_path):
+    """Files of two sizes: a chunk whose files share a size is one frames_in launch, a mixed chunk one per file.  Every
+    HMR input and every gt_ file is the cv2 route's, bit for bit."""
+    size = C.SIZE
+    frames = [world["frames"][0], world["frames"][1], world["frames"][2], F.frames(1, 120, 90, seed=12)[0]]
+    paths = []
+    for i, fr in enumerate(frames):                       # chunks of 2: (333x517, 333x517), (333x517, 120x90)
+        paths.append(str(tmp_path / ("t%d.png" % i)))
+        cv2.imwrite(paths[-1], fr)
+    out = tmp_path / "out"
+    out.mkdir()
+    hmr = RecordingHMR(world["v"])
+    im = Imitator(_opt(size), generator=world["net"], hmr=hmr, render=_render(world, size), device=cuda)
+    src_theta = np.zeros(85, np.float32)
+    src_theta[0] = 0.95
+    im.personalize(world["paths"][0], src_smpl=src_theta)
+    got = im.inference(paths, tgt_smpls=None, output_dir=str(out))
+    assert len(got) == 4 and len(hmr.inputs) == 2
+    hmr_in = torch.cat(hmr.inputs)
+    for i, fr in enumerate(frames):
+        _, r_hmr, r_gt = F.cv2_route(fr, size)
+        assert np.array_equal(_bits(hmr_in[i]), _bits(r_hmr)), i
+        ref = str(tmp_path / ("ref%d.png" % i))
+        cv2.imwrite(ref, r_gt)
+        assert open(str(out / ("gt_t%d.png" % i)), "rb").read() == open(ref, "rb").read(), i
+        assert os.path.exists(str(out / ("pred_t%d.png" % i)))
+    assert np.array_equal(im.tsf_info["image"], cv2.cvtColor(frames[-1], cv2.COLOR_BGR2RGB))
+
+
+def test_inference_with_given_smpls_reads_only_the_last_file(cuda, world, monkeypatch):
+    """Given SMPL vectors and no output_dir (evaluate.py's call): no file is decoded but the last one, for
+    tsf_info['image'], and the frames are those of inference_by_smpls."""
+    im = Imitator(_opt(), generator=world["net"], hmr=RecordingHMR(world["v"]), render=_render(world, C.SIZE), device=cuda)
+    im.personalize('', src_frame=world["frames"][0])
+    tgt = np.zeros((5, 85), np.float32)
+    tgt[:, 0], tgt[:, 3] = 0.9, [0, 1, 2, 3, 0]
+    reads, imread = [], cv2.imread
+    monkeypatch.setattr(cv2, "imread", lambda path, *a: reads.append(path) or imread(path, *a))
+    got = im.inference(world["paths"], tgt_smpls=list(tgt))
+    assert reads == [world["paths"][-1]]
+    assert np.array_equal(im.tsf_info["image"], cv2.cvtColor(world["frames"][-1], cv2.COLOR_BGR2RGB))
+    assert all(np.array_equal(a, b) for a, b in zip(got, im.inference_by_smpls(list(tgt))))
+
+
 def test_viewer_from_a_frame_equals_from_its_file(cuda, world):
     views = []
     for kind in ("path", "frame"):

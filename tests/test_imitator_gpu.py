@@ -283,3 +283,54 @@ def test_imitator_graph_replay_matches_eager(cuda, monkeypatch):
     for x, y in zip(results["0"][1], results["1"][1]):
         assert np.abs(x.astype(np.int32) - y.astype(np.int32)).max() <= 1
     assert torch.equal(results["0"][3], results["1"][3])
+
+
+def test_imitator_range_bits_redo_the_sequence_in_fp16x3_once(cuda, tmp_path, monkeypatch):
+    """Operand-range bits from a pass: the generator is pinned to fp16x3 and the sequence is computed once more (the
+    frames and files are that pass's, and its own bits are not checked again); LWB_AUTO_PRECISION=0 only warns, and
+    RANGE_FP16 raises.  The bits are forced through a stand-in for the generator's range flag."""
+    import warnings
+    from impersonator_b200._lib import LwbError
+    from impersonator_b200.binding import RANGE_FP16, RANGE_HEADS
+    torch.set_grad_enabled(False)
+    monkeypatch.delenv("LWB_PRECISION", raising=False)
+    monkeypatch.delenv("LWB_AUTO_PRECISION", raising=False)
+    size = 256
+    v, f = S.uv_sphere()
+    tabs = S.synthetic_tables()
+    net = ImpersonatorGenerator(bg_dim=4, src_dim=6, tsf_dim=6, repeat_num=6)
+    net.load_state_dict(S.fill_state_dict(net.state_dict(), seed=0))
+    im = Imitator(Opt(), generator=net, hmr=SyntheticBodyModel(v),
+                  render=SMPLRenderer(image_size=size, faces=f.numpy(), map_fn=tabs["map_fn"]), device=cuda)
+    src_theta = np.zeros(85, np.float32)
+    src_theta[0] = 0.95
+    im.personalize("", src_smpl=src_theta, src_img=S.synthetic_source(size))
+    tgt = np.zeros((3, 85), np.float32)
+    tgt[:, 0], tgt[:, 3] = 0.9, np.array([0.2, 1.0, -2.0])
+    flag = torch.full((1,), RANGE_HEADS, dtype=torch.int32, device=cuda)
+    monkeypatch.setattr(im.generator.tsf_model, "range_flag_tensor", lambda: flag)
+
+    def run(**kw):
+        with warnings.catch_warnings(record=True) as rec:
+            warnings.simplefilter("always")
+            outs = im.inference_by_smpls(list(tgt), **kw)
+        return outs, [str(w.message) for w in rec if "lwb_b200" in str(w.message)]
+
+    monkeypatch.setenv("LWB_AUTO_PRECISION", "0")
+    outs, said = run()
+    assert len(outs) == 3 and len(said) == 1 and "precision mode kept" in said[0]
+    assert getattr(net, "_lwb_precision", None) is None
+    monkeypatch.delenv("LWB_AUTO_PRECISION")
+    outs, said = run(output_dir=str(tmp_path))
+    assert len(outs) == 3 and len(said) == 1 and "switching this generator to LWB_PRECISION=fp16x3" in said[0]
+    assert getattr(net, "_lwb_precision", None) == "fp16x3"
+    flag.zero_()
+    clean, said = run()
+    assert said == [] and len(clean) == 3
+    for a, b in zip(outs, clean):
+        assert np.abs(a - b).max() < 1e-5
+    assert sorted(p.name for p in tmp_path.iterdir()) == ["pred_%.8d.jpg" % t for t in range(3)]
+    flag.fill_(RANGE_FP16)
+    net.set_precision(None)
+    with pytest.raises(LwbError, match="fp16 range"):
+        run()

@@ -1,7 +1,8 @@
 """Input path: decoded uint8 frames -> the Imitator's generator input (S x S) and HMR input (224 x 224), per frame at
-batch 16, through the host route the file path takes after cv2.imread and through lwb_frames_in.
+batch 16, through the reference's host route after cv2.imread and through lwb_frames_in, which the Imitator uses.
 
-  host    cvtColor + cv2.resize to S + cv2.resize to 224 + float conversion (x / 255 * 2 - 1) + H2D of both
+  host    the reference's computation: cvtColor + cv2.resize to S + cv2.resize to 224 + float conversion
+          (x / 255 * 2 - 1) + H2D of both
   device  pinned uint8 H2D of the frames + one lwb_frames_in launch
   kernel  lwb_frames_in alone (CUDA events over many launches), with the bytes it must move (each source byte read once,
           both float outputs written) over the kernel time, against the H100 SXM data-sheet HBM3 peak of 3.35 TB/s
@@ -42,7 +43,7 @@ def host_route(frames, size, dev):
         rgb = cv2.cvtColor(f, cv2.COLOR_BGR2RGB)
         img.append((cv2.resize(rgb, (size, size)).astype(np.float32) / 255.0).transpose((2, 0, 1)) * 2 - 1.0)
         hmr.append(cv2.resize(rgb, (224, 224)).astype(np.float32).transpose((2, 0, 1)) / 255.0 * 2 - 1.0)
-    a = torch.from_numpy(np.stack(img)).to(dev)                            # as Imitator's file route copies them
+    a = torch.from_numpy(np.stack(img)).to(dev)
     b = torch.from_numpy(np.stack(hmr)).to(dev)
     torch.cuda.synchronize()
     return a, b
